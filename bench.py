@@ -1,7 +1,8 @@
-"""bench.py -- CMVM solve throughput on B200 (BASELINE.json metric: 256x256 int8 matrices/s).
+"""bench.py -- CMVM solve throughput on the GPU (BASELINE.json metric: 256x256 int8 matrices/s).
 
     python bench.py --gpus N --steps K --warmup W            # CUDA path (this repository)
     python bench.py --impl reference --gpus N ...            # the reference's own CPU code (oracle/_ref)
+    python bench.py ... --dump-outputs DIR                   # also write what the last timed step returned, DIR/<name>.npy
 
 A "step" = one pass of the hot path over one batch: every rank solves ``--batch`` synthetic 256x256 int8 constant
 matrices with the reference's default call (``solve(W)``: search over all decompose_dc candidates, two CSE stages each).
@@ -18,6 +19,7 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 from pathlib import Path
@@ -29,6 +31,9 @@ sys.path.insert(0, str(ROOT))
 
 METRIC = 'cmvm_solve_throughput_256x256_int8'  # BASELINE.json metric (default workload)
 UNIT = 'matrices/s'
+STAGE_KEYS = ('inp_shifts', 'out_idxs', 'out_shifts', 'out_negs', 'ops_i', 'ops_f')
+HBM_PEAK_GBS = 3350.0  # NVIDIA H100 SXM data sheet, HBM3 (a card set below 700 W reaches less)
+DUMP_BYTES = 64 << 20
 
 
 def metric_name(n: int, bits: int) -> str:
@@ -71,9 +76,9 @@ def stage_digest(stages) -> str:
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region, with the card's name and power limit."""
 
-    QUERY = 'clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap'
+    QUERY = 'clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,name,power.limit'
 
     def __init__(self, index: int):
         self.index = index
@@ -106,7 +111,8 @@ class ClockSampler:
         sm = sorted(float(r[0]) for r in self.rows if r[0].replace('.', '').isdigit())
         names = ['hw_slowdown', 'hw_thermal_slowdown', 'sw_thermal_slowdown', 'sw_power_cap']
         reasons = [n for i, n in enumerate(names) if any(r[3 + i].lower().startswith('active') for r in self.rows if len(r) > 3 + i)]
-        return {'sm_mhz': sm[len(sm) // 2] if sm else None, 'sm_max_mhz': float(self.rows[0][1]) if self.rows[0][1].replace('.', '').isdigit() else None,
+        return {'gpu': self.rows[0][7] if len(self.rows[0]) > 8 else None, 'power_limit_w': self.rows[0][8] if len(self.rows[0]) > 8 else None,
+                'sm_mhz': sm[len(sm) // 2] if sm else None, 'sm_max_mhz': float(self.rows[0][1]) if self.rows[0][1].replace('.', '').isdigit() else None,
                 'power_w_max': max((float(r[2]) for r in self.rows if r[2].replace('.', '').isdigit()), default=None), 'reasons': reasons, 'samples': len(self.rows)}
 
 
@@ -117,20 +123,53 @@ def dist_env():
     return rank, world, local
 
 
+# algorithmic byte counts are a deterministic function of the workload; they are cached outside the tree (which may be
+# read-only) so that later runs, and the reference arm, skip the accounting passes
+ALGO_CACHE = Path(tempfile.gettempdir()) / 'da4ml_b200_bench' / 'algo_bytes.json'
+
+
 def cached_algo_bytes(key: str):
-    cache = ROOT / 'profiles' / 'algo_bytes.json'
-    return json.loads(cache.read_text()).get(key) if cache.exists() else None
+    try:
+        return json.loads(ALGO_CACHE.read_text()).get(key)
+    except (OSError, ValueError):
+        return None
 
 
 def store_algo_bytes(key: str, value: float):
-    cache = ROOT / 'profiles' / 'algo_bytes.json'
-    known = json.loads(cache.read_text()) if cache.exists() else {}
-    known[key] = value
     try:
-        cache.parent.mkdir(exist_ok=True)
-        cache.write_text(json.dumps(known, indent=1, sort_keys=True))
-    except OSError:
+        known = json.loads(ALGO_CACHE.read_text()) if ALGO_CACHE.exists() else {}
+        known[key] = value
+        ALGO_CACHE.parent.mkdir(parents=True, exist_ok=True)
+        tmp = ALGO_CACHE.with_name(f'.{ALGO_CACHE.name}.{os.getpid()}')
+        tmp.write_text(json.dumps(known, indent=1, sort_keys=True))
+        os.replace(tmp, ALGO_CACHE)
+    except (OSError, ValueError):
         pass
+
+
+def dump_outputs(out_dir: str, res, seeds, prefix: str = ''):
+    """Write the arrays the timed call returned (one RawPipeline per matrix: the stage arrays of the C ABI) as
+    ``<out_dir>/<prefix>m<i>_s<stage>_<key>.npy``, float64 (ops_f float32), with ``n_adders`` and the matrices' ``seeds``.
+    At most DUMP_BYTES in all: whole results in batch order while they fit; a first result that alone is larger is
+    written as a fixed seeded sample of its rows."""
+    out = Path(out_dir)
+    out.mkdir(parents=True, exist_ok=True)
+    arrays = {'n_adders': np.array([r.n_adders for r in res], np.float64), 'seeds': np.array(seeds, np.float64)}
+    budget = DUMP_BYTES - sum(a.nbytes for a in arrays.values())
+    for m, r in enumerate(res):
+        mine = {f'm{m}_s{s}_{k}': np.asarray(st[k], np.float32 if k == 'ops_f' else np.float64) for s, st in enumerate(r.stages) for k in STAGE_KEYS}
+        size = sum(a.nbytes for a in mine.values())
+        if size > budget:
+            if m > 0:
+                break
+            rng = np.random.default_rng(0)
+            for name, a in mine.items():
+                mine[name] = a[np.sort(rng.choice(len(a), size=int(len(a) * budget / size * 0.99), replace=False))]
+            size = sum(a.nbytes for a in mine.values())
+        arrays.update(mine)
+        budget -= size
+    for name, a in arrays.items():
+        np.save(out / f'{prefix}{name}.npy', a)
 
 
 def full_cpu_run(n: int, bits: int, seed: int = 0):
@@ -223,7 +262,7 @@ def run_reference(args):
         'e2e': {'value': value, 'unit': UNIT, 'h2d_bytes_per_step': 0, 'd2h_bytes_per_step': 0},
     }
     if a_total is None:
-        line['note'] = 'algorithmic bytes of the full solve unknown (run the CUDA arm once to cache profiles/algo_bytes.json); reporting bytes/s only'
+        line['note'] = 'algorithmic bytes of the full solve unknown (a run of the CUDA arm on this machine caches it); reporting bytes/s only'
         line['cpu_baseline']['algo_bytes_per_s'] = info['algo_bytes_per_s']
     print(json.dumps(line), flush=True)
     return 0
@@ -312,7 +351,7 @@ def run_cuda(args):
 
     # ---- timed region 1: inputs resident in HBM, CUDA events on the launching stream
     # (per-step working set: histogram segments, cell pools and op tables of the concurrent candidates, several hundred
-    #  MB, i.e. larger than the 126 MB L2, and every step solves NEW matrices: nothing of one step survives into the next)
+    #  MB, i.e. larger than the 50 MB L2, and every step solves NEW matrices: nothing of one step survives into the next)
     launches = 0
     solve_ms = 0.0
     solve_launches = 0
@@ -345,6 +384,8 @@ def run_cuda(args):
             if not ok:
                 mismatches.append(seed)
     adders = [[r.n_adders for r in res] for res in results]
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, results[-1], step_seeds(args.steps - 1), f'r{rank}_' if world > 1 else '')
     # ---- timed region 2 (end to end): host numpy in -> the reference's result type (Pipeline of CombLogic / Op) out,
     # through the public call a user makes (da4ml_b200.cmvm.solve / solve_batch); and the same down to flat arrays only
     barrier()
@@ -407,8 +448,7 @@ def run_cuda(args):
                 d4 = torch.from_numpy(c4_mats[0]).to(dev)
                 a4 = accounting_bytes(B, d4.data_ptr(), (128, 128), share=True)
                 store_algo_bytes('128x128_int6_default_seed0', a4)
-            peaks = json.loads((ROOT / 'MEASURED_PEAKS.json').read_text()) if (ROOT / 'MEASURED_PEAKS.json').exists() else {}
-            pk = float(peaks.get('hbm_gbs', 6650.0))
+            pk = HBM_PEAK_GBS
             ach = a4 * args.c4 / c4_time / 1e9
             c4['roofline'] = {'bound': 'hbm', 'achieved': ach, 'peak': pk, 'unit': 'GB/s', 'frac': ach / pk,
                               'note': 'algorithmic bytes of seed 0 (exact, accounting mode) x 64 matrices / end-to-end wall time of the job'}
@@ -421,19 +461,11 @@ def run_cuda(args):
     value = total / (dev_ms_max * 1e-3)
 
     if rank == 0:
-        peaks = {}
-        pk = ROOT / 'MEASURED_PEAKS.json'
-        if pk.exists():
-            peaks = json.loads(pk.read_text())
-        peak_gbs = float(peaks.get('hbm_gbs', 6650.0))
-        peak_src = 'measured (MEASURED_PEAKS.json hbm_gbs)' if 'hbm_gbs' in peaks else 'fallback 6.65 TB/s'
+        peak_gbs = HBM_PEAK_GBS
+        peak_src = 'NVIDIA H100 SXM data sheet (HBM3), not measured'
         # dominant kernel: the persistent solve kernel.  Algorithmic bytes of everything those launches solved / their CUDA-event time.
         a_step = (a_run or 0.0) * args.batch
         achieved = (a_step * args.steps) / (solve_ms * 1e-3) / 1e9 if solve_ms > 0 else None
-        traffic = None
-        tj = ROOT / 'profiles' / 'traffic.json'
-        if tj.exists():
-            traffic = json.loads(tj.read_text()).get('solve_kernel_dram_bytes_per_launch')
         cpu = cpu_sample(n, bits, args.seed, a_ref, args.cpu_seconds, 1) if args.cpu_seconds > 0 else None
         line = {
             'metric': metric_name(n, bits), 'value': value, 'unit': UNIT, 'n_gpus': world, 'steps': args.steps, 'warmup': args.warmup,
@@ -441,7 +473,7 @@ def run_cuda(args):
             'dtype': 'u32 sign planes / f32 intervals', 'data': 'synthetic',
             'config': {
                 'workload': workload_name(n, bits, args.batch) if args.total <= 0 else f'{n}x{n} int{bits} default solve(), fixed job of {args.total} matrices over {world} rank(s)',
-                'timing': 'every step solves new matrices and the per-step working set (histogram segments, cell pools, op tables of the concurrent candidates) exceeds the 126 MB L2',
+                'timing': 'every step solves new matrices and the per-step working set (histogram segments, cell pools, op tables of the concurrent candidates) exceeds the 50 MB L2',
                 'adders_rank0': adders,
                 'jobs': {'reference_solve_single_calls': jobs_total, 'executed': jobs_run,
                          'note': 'byte-identical solve_single jobs of one call (decompose_dc candidates with the same stage matrix) are solved once'},
@@ -456,7 +488,7 @@ def run_cuda(args):
             'e2e_raw': {'value': total / (e2e_raw_ms_max * 1e-3), 'unit': UNIT, 'ms_per_step': e2e_raw_ms_max / args.steps, 'what': 'the same down to the flat result arrays of the C ABI (no Python containers)'},
             'roofline': {
                 'bound': 'hbm', 'kernel': 'cmvm_solve_kernel', 'achieved': achieved, 'peak': peak_gbs, 'unit': 'GB/s',
-                'frac': (achieved / peak_gbs) if achieved else None, 'traffic': traffic, 'traffic_source': 'static: one ncu --set full capture (profiles/traffic.json), not measured in this run',
+                'frac': (achieved / peak_gbs) if achieved else None,
                 'peak_source': peak_src, 'algo_bytes_per_step': a_step, 'algo_bytes_per_step_reference': (a_ref or 0.0) * args.batch,
                 'launches_per_step': solve_launches / max(1, args.steps), 'kernel_ms_per_step': solve_ms / max(1, args.steps),
                 # SURVEY 8d defines A over every solve_single the REFERENCE executes for the call; `frac` above is the stricter figure
@@ -495,6 +527,7 @@ def main():
     ap.add_argument('--c4', type=int, default=64, help='matrices of the BASELINE config 4 sub-record (128x128 int6, fixed job over the ranks); 0 disables')
     ap.add_argument('--cpu-seconds', type=float, default=15.0, help='bounded CPU-baseline sample (0 disables)')
     ap.add_argument('--recount', action='store_true', help='recompute the cached algorithmic-byte figures')
+    ap.add_argument('--dump-outputs', metavar='DIR', help='after the timed steps, write what the last one returned as DIR/<name>.npy (at most 64 MB)')
     args = ap.parse_args()
     if args.impl == 'reference':
         return run_reference(args)

@@ -1,4 +1,4 @@
-"""da4ml_b200 -- B200-native (sm_100a CUDA) CMVM distributed-arithmetic solver.
+"""da4ml_b200 -- GPU-native (sm_90a CUDA, H100) CMVM distributed-arithmetic solver.
 
 Drop-in for the ``da4ml.cmvm.solve`` path of calad0i/da4ml; see DESIGN.md / INTEGRATION.md.
 """

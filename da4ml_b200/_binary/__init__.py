@@ -21,7 +21,7 @@ _LIB_PATH = Path(__file__).resolve().parent / 'libda4ml_b200_cmvm.so'
 if not _LIB_PATH.exists():
     raise ImportError(
         f'{_LIB_PATH} not found: build it with `python -c "import __graft_entry__ as g; g.build()"` '
-        '(nvcc, sm_100a). The CMVM solver has no CPU fallback.'
+        '(nvcc, sm_90a). The CMVM solver has no CPU fallback.'
     )
 _L = C.CDLL(str(_LIB_PATH))
 
@@ -99,7 +99,7 @@ PLAN_FIELDS = ['ctas_per_problem', 'concurrent_groups', 'columns_per_cta', 'list
                'segment_entries_per_cta', 'log2_pair_counters', 'shared_bytes', 'shared_budget', 'narrow_rows', 'spill_rows']
 
 
-def plan(jobs, co_resident_ctas: int = 148, group_override: int = 0) -> dict:
+def plan(jobs, co_resident_ctas: int = 132, group_override: int = 0) -> dict:
     """Launch geometry the solver would pick for ``jobs`` (no device needed).  Each job is a dict with ``n_in, n_out,
     nbits, digits`` (CSD digits of the matrix) and optionally ``dcol_max`` (digits of the densest column, default
     digits / n_out), ``col_cap`` (bound on rows per column list, default n_in + dcol_max), ``f_mul, list_mul``

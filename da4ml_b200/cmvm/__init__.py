@@ -1,7 +1,7 @@
 """``da4ml_b200.cmvm`` -- the public face of the solver, name-compatible with the reference's ``da4ml.cmvm``
 (reference ``src/da4ml/cmvm/__init__.py``: ``solve``, ``kernel_decompose``, ``QInterval``, ``Op``, ``CombLogic`` and the
 ``solver_options_t`` keyword bundle that tracing code splats into ``solve``).  ``solve_batch`` / ``solve_calls`` are the
-B200-side additions for many independent matrices."""
+GPU-side additions for many independent matrices."""
 
 from typing import TypedDict
 

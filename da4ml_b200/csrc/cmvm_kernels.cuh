@@ -1,4 +1,4 @@
-// cmvm_kernels.cuh -- sm_100a kernels of the CMVM greedy common-subexpression solver.
+// cmvm_kernels.cuh -- sm_90a kernels of the CMVM greedy common-subexpression solver.
 //
 //   cmvm_prep_kernel    centre + CSD-decompose the constant matrix into packed sign planes
 //                       (bit_decompose.hh:21-34, bit_decompose.cc:22-62, state_opr.cc:92-97)

@@ -1,4 +1,4 @@
-// cmvm_lib.cu -- host driver and C ABI (include/da4ml_b200_cmvm.h) of the B200-native CMVM solver.
+// cmvm_lib.cu -- host driver and C ABI (include/da4ml_b200_cmvm.h) of the GPU-native CMVM solver.
 //
 // Host-side control mirrors the reference's api.cc: `solve` (candidate search over decompose_dc,
 // api.cc:147-250) and `_solve` (two-stage driver with the latency-retry loop, api.cc:28-145).  The

@@ -20,7 +20,7 @@ struct PlanJob {
     int e_cap = 0;               // expression ids the job may use
 };
 struct PlanEnv {
-    int coop = 148;      // co-resident CTAs of the launch (one persistent 512-thread CTA per SM)
+    int coop = 132;      // co-resident CTAs of the launch (one persistent 512-thread CTA per SM of an H100 SXM)
     bool accounting = false;
     int group_override = 0; // > 0: fixed group size (set_group_size)
     long long own_budget = 208 * 1024; // dynamic shared memory one CTA of the solve kernel may use
@@ -118,10 +118,10 @@ inline LaunchPlan plan_launch(const std::vector<PlanJob> &jobs, const PlanEnv &e
     const int groups = (n + waves - 1) / waves;
     G = (int)std::min<long long>(want, std::max(G, coop / groups));
     if (waves > 1) {
-        // Several waves of (nearly) equal jobs: a job's time is ~ 1 / G in this range (measured: 128x128 int6 stage, G = 2, 3,
-        // 4 -> 67.6, 46.7, 34.2 us per step), so the launch costs ceil(n / floor(coop / G)) / G job-times: pick the group size
-        // that wastes the least of the last wave (64 x config 4: 384 jobs, G = 2 -> 6 waves on 74 groups = 0.865 of the
-        // CTAs busy; G = 3 -> 8 waves on 49 groups = 0.973).  Ties go to the smaller group.
+        // Several waves of (nearly) equal jobs: a job's time is ~ 1 / G in this range, so the launch costs
+        // ceil(n / floor(coop / G)) / G job-times: pick the group size that wastes the least of the last wave (64 x config 4:
+        // 384 jobs on 148 CTAs, G = 2 -> 6 waves on 74 groups = 0.865 of the CTAs busy; G = 3 -> 8 waves on 49 groups = 0.973).
+        // Ties go to the smaller group.
         const int g_lo = G, g_hi = (int)std::min<long long>(want, 2LL * G + 2);
         double best_u = 0.0;
         for (int g = g_lo; g <= g_hi; ++g) {

@@ -40,7 +40,7 @@ int da4ml_cmvm_set_stream(void *cuda_stream);
 /* Tuning knob: CTAs cooperating on one problem (0 = automatic). */
 int da4ml_cmvm_set_group_size(int ctas_per_problem);
 
-/* Launch geometry the solver would choose for a set of solve_single jobs on `co_resident_ctas` CTAs (148 on a B200),
+/* Launch geometry the solver would choose for a set of solve_single jobs on `co_resident_ctas` CTAs (132 on an H100 SXM),
  * without touching a device.  jobs: [n][8] int64 = {n_in, n_out, nbits, csd_digits, max_digits_per_column,
  * column_list_bound, f_mul, list_mul}; out: [12] int64 = {ctas_per_problem, concurrent_groups, columns_per_cta (adder
  * trees), list_rows_in_shared_memory, log2_chunk, chunk_slots, segment_entries_per_cta, log2_pair_counters,

@@ -13,7 +13,7 @@ STAGE_KEYS = ['inp_shifts', 'out_idxs', 'out_shifts', 'out_negs', 'ops_i', 'ops_
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box with -m gpu)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (select with -m gpu)')
 
 
 def int_matrix(n_in, n_out, bits, seed):

@@ -1,14 +1,35 @@
-"""SURVEY 8f N2: replay of the adder graphs with the DAIS int64 semantics.  CPU: the compiled reference interpreter
-(oracle/_ref/libdais_ref.so) agrees with the float replay on in-range inputs.  GPU: the CUDA replay equals the reference
-interpreter bit for bit, including the wrap-around of out-of-range inputs."""
+"""SURVEY 8f N2: replay of the adder graphs with the DAIS int64 semantics.  CPU: the reference's DAIS interpreter
+agrees with the float replay on in-range inputs.  GPU: the CUDA replay equals the reference interpreter bit for bit,
+including the wrap-around of out-of-range inputs.  What the reference interpreter returned for these programs and inputs
+is stored in tests/golden/dais_reference.json.gz (tests/golden/make_golden_refchecks.py)."""
+import hashlib
+
 import numpy as np
 import pytest
 from conftest import golden_cases, int_matrix, load_golden
 
 from da4ml_b200.types import pipeline_from_arrays
-from oracle import dais_ref
 
-needs_ref = pytest.mark.skipif(not dais_ref.available(), reason='oracle/_ref/libdais_ref.so not built')
+
+def run_key(program, data) -> str:
+    """Key of one interpreter run in the stored file: digest of the program words and the float64 inputs."""
+    h = hashlib.sha256(np.ascontiguousarray(program, dtype=np.int32).tobytes())
+    h.update(np.ascontiguousarray(data, dtype=np.float64).tobytes())
+    return 'run_' + h.hexdigest()
+
+
+@pytest.fixture(scope='module')
+def dais_want():
+    from test_oracle_cross import load_stored
+
+    return load_stored('dais_reference.json.gz')
+
+
+def reference_run(z, program, data):
+    """The reference interpreter's output for ``program`` on ``data``, as stored."""
+    key = run_key(program, data)
+    assert key in z, 'no stored reference output for this program and input (regenerate tests/golden/dais_reference.json.gz)'
+    return z[key]
 
 
 def golden_stage_programs():
@@ -23,37 +44,50 @@ def golden_stage_programs():
     return out
 
 
-@needs_ref
-def test_reference_interpreter_agrees_with_float_replay():
+def float_replay_inputs():
     rng = np.random.default_rng(0)
     for tag, sol in golden_stage_programs():
         if '/s0' not in tag or 'hetero' in tag:
             continue  # stage-0 graphs with the default 8-bit inputs: every sample is in range
-        x = rng.integers(-128, 128, size=(9, sol.shape[0])).astype(np.float64)
-        assert np.array_equal(dais_ref.run(sol.to_binary(), x), sol(x)), tag
+        yield tag, sol, rng.integers(-128, 128, size=(9, sol.shape[0])).astype(np.float64)
 
 
-@needs_ref
-@pytest.mark.gpu
-def test_cuda_replay_matches_reference_interpreter(cuda_binary):
+def cuda_replay_inputs():
     rng = np.random.default_rng(1)
     for tag, sol in golden_stage_programs():
         n_in = sol.shape[0]
-        x = np.concatenate([rng.integers(-128, 128, size=(33, n_in)), rng.integers(-5000, 5000, size=(8, n_in)) / 8.0]).astype(np.float64)
-        want = dais_ref.run(sol.to_binary(), x)
+        yield tag, sol, np.concatenate([rng.integers(-128, 128, size=(33, n_in)), rng.integers(-5000, 5000, size=(8, n_in)) / 8.0]).astype(np.float64)
+
+
+SOLVED_W = (64, 48, 8, 21)  # int_matrix arguments of test_cuda_replay_of_a_solved_matrix
+
+
+def solved_matrix_inputs():
+    return np.random.default_rng(2).integers(-128, 128, size=(5000, 64)).astype(np.float64)
+
+
+def test_reference_interpreter_agrees_with_float_replay(dais_want):
+    for tag, sol, x in float_replay_inputs():
+        assert np.array_equal(reference_run(dais_want, sol.to_binary(), x), sol(x)), tag
+
+
+@pytest.mark.gpu
+def test_cuda_replay_matches_reference_interpreter(cuda_binary, dais_want):
+    for tag, sol, x in cuda_replay_inputs():
+        want = reference_run(dais_want, sol.to_binary(), x)
         got = sol.predict(x)
         assert got.dtype == np.float64 and np.array_equal(got.view(np.uint64), want.view(np.uint64)), tag
 
 
-@needs_ref
 @pytest.mark.gpu
-def test_cuda_replay_of_a_solved_matrix(cuda_binary):
-    W = int_matrix(64, 48, 8, 21)
+def test_cuda_replay_of_a_solved_matrix(cuda_binary, dais_want):
+    W = int_matrix(*SOLVED_W)
     pipe = cuda_binary.solve(W, search_all_decompose_dc=False, decompose_dc=-1)
     sol = pipe.solutions[0]
-    x = np.random.default_rng(2).integers(-128, 128, size=(5000, 64)).astype(np.float64)
+    x = solved_matrix_inputs()
     got = sol.predict(x)
-    assert np.array_equal(got, dais_ref.run(sol.to_binary(), x))
+    # (the reference's output for 5000 samples is stored as the sha256 of its float64 bytes)
+    assert got.dtype == np.float64 and hashlib.sha256(np.ascontiguousarray(got).tobytes()).hexdigest() == dais_want['solved_sha256']
     assert np.array_equal(got, sol(x))  # in-range inputs: fixed-point replay == exact arithmetic
     with pytest.raises(RuntimeError, match='Unknown opcode'):
         bad = sol.to_binary()
@@ -74,13 +108,12 @@ def _raw_from_golden(name):
     return B.RawPipeline.from_stages(stages), want
 
 
-@needs_ref
-def test_kernel_from_fixed_point_probes(monkeypatch):
+def test_kernel_from_fixed_point_probes(monkeypatch, dais_want):
     """``RawPipeline.kernel`` probes every stage with one quantum per input under the DAIS fixed-point semantics; with
     the reference interpreter standing in for the CUDA one, it reproduces the matrix of every golden case."""
     import da4ml_b200._binary as B
 
-    monkeypatch.setattr(B, 'dais_interp_run', lambda prog, x, n_threads=1: dais_ref.run(prog, x))
+    monkeypatch.setattr(B, 'dais_interp_run', lambda prog, x, n_threads=1: reference_run(dais_want, prog, x))
     for name in golden_cases():
         raw, want = _raw_from_golden(name)
         assert np.array_equal(raw.kernel, want), name

@@ -135,7 +135,7 @@ def test_foreign_opcodes_are_rejected():
 @pytest.mark.gpu
 @pytest.mark.parametrize('name', ['c1_8x8_int4_default', 'int_16x16_int8_default', 'pytest_8_b4_harddc2_add1', 'int_12x20_int6_harddc1'])
 def test_gpu_result_arrays_emit_the_reference_text(cuda_binary, gold, name):
-    """The whole chain on the B200: CUDA solve -> flat arrays -> pipelining / emitters, no Op objects in between; the text
+    """The whole chain on the GPU: CUDA solve -> flat arrays -> pipelining / emitters, no Op objects in between; the text
     equals what the reference's emitters write for the reference's own solve of the same matrix."""
     meta = golden_cases()[name]
     extra, _ = load_golden(name)
@@ -190,30 +190,3 @@ def test_retiming_matches_the_reference_tracer(gold, name):
         _same_stages(emit.to_pipeline(stages[0], float(cut), retiming=True), want['retimed'])
         n_checked += 1
     assert n_checked > 0
-
-
-@pytest.mark.skipif(not __import__('pathlib').Path('/root/reference/src/da4ml/trace').exists(), reason='needs the reference tree (build container)')
-def test_retiming_is_delegated_to_the_reference_tracer():
-    """``retiming=True, da4ml=<package>`` hands the split to the reference's own ``retime_pipeline`` and returns flat stages
-    (the route for graphs in which the tracer produces constants); equal to the reference's ``to_pipeline(..., retiming=True)``
-    and, for this constant-free graph, to the native retiming."""
-    import importlib
-    import sys
-
-    import ref_trace
-    from oracle import port
-
-    T, _ = ref_trace.load(None, port.get_lsb_loc, port.iceil_log2, port.cost_add)
-    P = importlib.import_module('da4ml.trace.pipeline')
-    st = _stages('pytest_8_b4_harddc2_add1')[0]
-    comb = pipeline_from_arrays([st], types_module=T).solutions[0]
-    for cut in (2.0, 3.0):
-        want = P.to_pipeline(comb, cut, retiming=True, verbose=False)
-        got = emit.to_pipeline(st, cut, retiming=True, da4ml=sys.modules['da4ml'])
-        native = emit.to_pipeline(st, cut, retiming=True)
-        assert len(got) == len(want.solutions) == len(native)
-        assert all(np.array_equal(a['ops_i'], b['ops_i']) and np.array_equal(a['ops_f'], b['ops_f']) for a, b in zip(got, native))
-        for a, b in zip(got, want.solutions):
-            assert a['ops_i'].tolist() == [[o.id0, o.id1, o.opcode, o.data] for o in b.ops]
-            assert a['ops_f'].tolist() == [[*o.qint, o.latency, o.cost] for o in b.ops]
-            assert a['out_idxs'].tolist() == list(b.out_idxs) and tuple(a['shape']) == tuple(b.shape)

@@ -2,8 +2,7 @@
 (``da4ml.trace.FixedVariableArray.matmul``, trace/fixed_variable_array.py:361-373: a Python loop over the left-hand rows,
 each calling ``cmvm()`` -> ``solve(W, qintervals=row intervals, latencies=row latencies, **solver_options)``) through
 ``SolveBatcher``: all rows in ONE batched GPU solve, identical rows solved once.  Every row's adder graph is compared with the
-call-by-call CUDA result and with the CPU checker.  The reference front-end itself is driven through the same batcher in
-tests/test_n1_reference_trace.py (CPU, build container: the reference tree does not exist on the GPU box)."""
+call-by-call CUDA result and with the CPU checker."""
 import numpy as np
 import pytest
 from conftest import assert_stage_equal, int_matrix

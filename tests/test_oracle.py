@@ -4,7 +4,7 @@ import json
 
 import numpy as np
 import pytest
-from conftest import GOLDEN, assert_stage_equal, golden_cases, int_matrix, load_golden
+from conftest import GOLDEN, STAGE_KEYS, assert_stage_equal, golden_cases, int_matrix, load_golden
 
 from oracle import port, ref
 
@@ -32,7 +32,7 @@ def test_port_matches_golden_single(name):
     assert got['counters']['sum_F'] == int(extra['f_sizes'].sum())
 
 
-@pytest.mark.skipif(not ref.available(), reason='oracle/_ref not built (needs /root/reference)')
+@pytest.mark.skipif(not ref.available(), reason='oracle/_ref not built (needs the reference sources)')
 @pytest.mark.parametrize('name', SOLVE_CASES)
 def test_reference_matches_golden(name):
     extra, stages = load_golden(name)
@@ -41,9 +41,7 @@ def test_reference_matches_golden(name):
         assert_stage_equal(a, b, f'{name} stage{i} ')
 
 
-@pytest.mark.skipif(not ref.available(), reason='oracle/_ref not built (needs /root/reference)')
-@pytest.mark.parametrize('seed', range(6))
-def test_port_matches_reference_random(seed):
+def random_case(seed):
     rng = np.random.default_rng(100 + seed)
     n_in, n_out, bits = int(rng.integers(2, 20)), int(rng.integers(2, 20)), int(rng.integers(2, 9))
     W = int_matrix(n_in, n_out, bits, seed)
@@ -56,9 +54,20 @@ def test_port_matches_reference_random(seed):
         carry_size=int(rng.choice([-1, 2, 8])),
         search_all_decompose_dc=bool(rng.integers(0, 2)),
     )
-    a, b = ref.solve(W, **kw), port.solve(W, **kw)
-    for i, (x, y) in enumerate(zip(a, b, strict=True)):
-        assert_stage_equal(x, y, f'{kw} stage{i} ')
+    return W, kw
+
+
+@pytest.mark.parametrize('seed', range(6))
+def test_port_matches_reference_random(seed):
+    """Against the reference's answers for these inputs, stored in tests/golden/reference_checks.json.gz."""
+    from test_oracle_cross import load_stored
+
+    z = load_stored('reference_checks.json.gz')
+    W, kw = random_case(seed)
+    b = port.solve(W, **kw)
+    assert len(b) == 2
+    for i, y in enumerate(b):
+        assert_stage_equal(y, {k: z[f'random{seed}_s{i}_{k}'] for k in STAGE_KEYS}, f'{kw} stage{i} ')
 
 
 @pytest.mark.parametrize('n,bits', [(2, 2), (4, 4), (8, 8)])

@@ -1,13 +1,12 @@
-"""The independent restatement (oracle/port) against the reference's own object code (oracle/_ref) on a broad random
-family of inputs: ragged shapes, sparse / scaled / wide matrices, heterogeneous intervals and latencies, every
-selector.  This is what lets the port stand in as the checker on a box where oracle/_ref is absent.  No GPU."""
+"""The independent restatement (oracle/port) against the reference's own object code on a broad random family of
+inputs: ragged shapes, sparse / scaled / wide matrices, heterogeneous intervals and latencies, every selector.  This is
+what lets the port stand in as the checker where the reference is absent.  The reference's answers for these inputs are
+stored in tests/golden/reference_checks.json.gz (tests/golden/make_golden_refchecks.py).  No GPU."""
 import numpy as np
 import pytest
-from conftest import assert_stage_equal
+from conftest import GOLDEN, assert_stage_equal
 
-from oracle import port, ref
-
-pytestmark = pytest.mark.skipif(not ref.available(), reason='oracle/_ref not built (needs /root/reference)')
+from oracle import port
 
 METHODS = ['mc', 'wmc', 'mc-dc', 'mc-pdc', 'wmc-dc', 'wmc-pdc']
 
@@ -64,8 +63,7 @@ def shapes(rng):
     return int(rng.integers(2, 22)), int(rng.integers(2, 22))
 
 
-@pytest.mark.parametrize('seed', range(60))
-def test_single_stage_random_family(seed):
+def single_case(seed):
     rng = np.random.default_rng(7000 + seed)
     n_in, n_out = shapes(rng)
     W, kind = random_matrix(rng, n_in, n_out)
@@ -76,11 +74,10 @@ def test_single_stage_random_family(seed):
         adder_size=int(rng.choice([-1, 1, 3, 8])),
         carry_size=int(rng.choice([-1, 1, 4])),
     )
-    assert_stage_equal(ref.solve_single(W, **kw), port.solve_single(W, **kw), f'{kind} {W.shape} {kw["method"]} ')
+    return W, kind, kw
 
 
-@pytest.mark.parametrize('seed', range(40))
-def test_full_solve_random_family(seed):
+def full_case(seed):
     rng = np.random.default_rng(9000 + seed)
     n_in, n_out = shapes(rng)
     W, kind = random_matrix(rng, n_in, n_out)
@@ -95,25 +92,67 @@ def test_full_solve_random_family(seed):
         carry_size=int(rng.choice([-1, 3])),
         search_all_decompose_dc=bool(rng.integers(0, 2)),
     )
-    a, b = ref.solve(W, **kw), port.solve(W, **kw)
-    assert len(a) == len(b) == 2
-    for i, (x, y) in enumerate(zip(a, b)):
-        assert_stage_equal(x, y, f'{kind} {W.shape} {kw} stage{i} ')
+    return W, kind, kw
 
 
-@pytest.mark.parametrize('seed', range(20))
-def test_helpers_random_family(seed):
+def helper_case(seed):
+    """(W, int32 values for int_arr_to_csd, integer-grid matrix for kernel_decompose)"""
     rng = np.random.default_rng(11000 + seed)
     n_in, n_out = shapes(rng)
     W, _ = random_matrix(rng, n_in, n_out)
-    for center in (True, False):
-        a, b = ref.csd_decompose(W, center), port.csd_decompose(W, center)
-        for x, y in zip(a, b):
-            assert x.shape == y.shape and np.array_equal(x, y)
     ints = rng.integers(-(2**20), 2**20, size=(int(rng.integers(1, 40)),)).astype(np.int32)
-    assert np.array_equal(ref.int_arr_to_csd(ints), port.int_arr_to_csd(ints))
     Wi = np.round(W * 64).astype(np.float32)  # kernel_decompose works on the integer grid
-    for dc in (-2, -1, 0, 1, 2):
-        a, b = ref.kernel_decompose(Wi, dc), port.kernel_decompose(Wi, dc)
+    return W, ints, Wi
+
+
+HELPER_DCS = (-2, -1, 0, 1, 2)
+
+
+def load_stored(name):
+    """A file written by tests/golden/make_golden_refchecks.py: name -> array (or digest string)."""
+    import gzip
+    import json
+
+    with gzip.open(GOLDEN / name, 'rt') as f:
+        return {k: v if isinstance(v, str) else np.asarray(v[2], dtype=v[0]).reshape(v[1]) for k, v in json.load(f).items()}
+
+
+@pytest.fixture(scope='module')
+def want():
+    return load_stored('reference_checks.json.gz')
+
+
+def stored_stage(z, prefix):
+    return {k: z[f'{prefix}_{k}'] for k in ('inp_shifts', 'out_idxs', 'out_shifts', 'out_negs', 'ops_i', 'ops_f')}
+
+
+@pytest.mark.parametrize('seed', range(60))
+def test_single_stage_random_family(want, seed):
+    W, kind, kw = single_case(seed)
+    assert_stage_equal(port.solve_single(W, **kw), stored_stage(want, f'cross_single{seed}'), f'{kind} {W.shape} {kw["method"]} ')
+
+
+@pytest.mark.parametrize('seed', range(40))
+def test_full_solve_random_family(want, seed):
+    W, kind, kw = full_case(seed)
+    b = port.solve(W, **kw)
+    assert len(b) == 2
+    for i, y in enumerate(b):
+        assert_stage_equal(y, stored_stage(want, f'cross_full{seed}_s{i}'), f'{kind} {W.shape} {kw} stage{i} ')
+
+
+@pytest.mark.parametrize('seed', range(20))
+def test_helpers_random_family(want, seed):
+    W, ints, Wi = helper_case(seed)
+    p = f'cross_helpers{seed}'
+    for center in (True, False):
+        b = port.csd_decompose(W, center)
+        for j, y in enumerate(b):
+            x = want[f'{p}_csd{int(center)}_{j}']
+            assert x.shape == y.shape and np.array_equal(x, y)
+    assert np.array_equal(want[f'{p}_ints_csd'], port.int_arr_to_csd(ints))
+    for dc in HELPER_DCS:
+        b = port.kernel_decompose(Wi, dc)
+        a = (want[f'{p}_kd{dc}_0'], want[f'{p}_kd{dc}_1'])
         assert np.array_equal(a[0], b[0]) and np.array_equal(a[1], b[1]), dc
         assert np.array_equal(a[0].astype(np.float64) @ a[1].astype(np.float64), Wi)

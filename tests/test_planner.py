@@ -26,8 +26,8 @@ def check_invariants(p, jobs, coop):
 
 def test_lone_problem_gets_the_whole_gpu():
     p = B.plan([job(256, 256, 8)])
-    check_invariants(p, [job(256, 256, 8)], 148)
-    assert p['ctas_per_problem'] == 148 and p['concurrent_groups'] == 1
+    check_invariants(p, [job(256, 256, 8)], 132)
+    assert p['ctas_per_problem'] == 132 and p['concurrent_groups'] == 1
     assert p['columns_per_cta'] == 2 and p['list_rows_smem'] > 0 and p['narrow_rows'] == 1
     tiny = B.plan([job(8, 8, 4)])
     assert tiny['ctas_per_problem'] == 1  # 100 digits cannot keep more than one CTA busy
@@ -38,17 +38,17 @@ def test_lone_problem_gets_the_whole_gpu():
 def test_candidates_of_one_call_share_the_gpu_in_one_wave():
     jobs = [job(256, 256, 8) for _ in range(10)]  # the ten decompose_dc candidates of the bench workload (before identical ones are shared)
     p = B.plan(jobs)
-    check_invariants(p, jobs, 148)
-    assert p['ctas_per_problem'] == 14 and p['concurrent_groups'] == 10
-    assert p['list_rows_smem'] >= 19 + 9 + 8 and p['log2_pair_counters'] == 13  # an owner's share of a column with slack, next to the large table
+    check_invariants(p, jobs, 132)
+    assert p['ctas_per_problem'] == 13 and p['concurrent_groups'] == 10
+    assert p['list_rows_smem'] >= 20 + 10 + 8 and p['log2_pair_counters'] == 13  # an owner's share of a column with slack, next to the large table
     six = B.plan(jobs[:6])
-    assert six['ctas_per_problem'] == 24 and six['concurrent_groups'] == 6
+    assert six['ctas_per_problem'] == 22 and six['concurrent_groups'] == 6
 
 
 def test_more_jobs_than_groups_run_in_equal_waves():
     jobs = [job(128, 128, 6) for _ in range(64)]
     p = B.plan(jobs)
-    check_invariants(p, jobs, 148)
+    check_invariants(p, jobs, 132)
     G, groups = p['ctas_per_problem'], p['concurrent_groups']
     waves = -(-len(jobs) // groups)
     assert waves * groups < len(jobs) + groups  # no nearly-empty last wave
@@ -56,25 +56,30 @@ def test_more_jobs_than_groups_run_in_equal_waves():
 
 
 def test_several_waves_pick_the_group_size_that_wastes_least_of_the_last_wave():
-    # BASELINE config 4 on one GPU: 64 matrices x 6 distinct stage-0 jobs.  2 CTAs per job would be 6 waves on 74 groups
-    # (0.865 of the CTA-time busy), 3 CTAs are 8 waves on 49 groups (0.973); a job's time is ~ 1 / G in this range.
+    # BASELINE config 4 on one H100 (132 SMs): 64 matrices x 6 distinct stage-0 jobs.  2 CTAs per job are 6 waves on 66
+    # groups (0.970 of the CTA-time busy), no larger group does better (3: 9 waves on 44 groups, 0.970; 7: 22 waves on 18
+    # groups, 0.926), and ties go to the smaller group; a job's time is ~ 1 / G in this range.
     jobs = [job(128, 128, 6) for _ in range(384)]
     p = B.plan(jobs)
-    check_invariants(p, jobs, 148)
+    check_invariants(p, jobs, 132)
     G, groups = p['ctas_per_problem'], p['concurrent_groups']
-    assert (G, groups) == (3, 49)
+    assert (G, groups) == (2, 66)
     waves = -(-len(jobs) // groups)
-    assert len(jobs) * G / (waves * 148) > 0.95
-    # a single wave is left alone (the default solve: 6 jobs x 24 CTAs), and so is a pinned group size
-    assert B.plan([job(256, 256, 8)] * 6)['ctas_per_problem'] == 24
+    assert len(jobs) * G / (waves * 132) > 0.95
+    # ... with 148 co-resident CTAs 2 CTAs per job would be 6 waves on 74 groups (0.865), 3 CTAs 8 waves on 49 groups (0.973)
+    p148 = B.plan(jobs, co_resident_ctas=148)
+    check_invariants(p148, jobs, 148)
+    assert (p148['ctas_per_problem'], p148['concurrent_groups']) == (3, 49)
+    # a single wave is left alone (the default solve: 6 jobs x 22 CTAs), and so is a pinned group size
+    assert B.plan([job(256, 256, 8)] * 6)['ctas_per_problem'] == 22
     assert B.plan(jobs, group_override=2)['ctas_per_problem'] == 2
 
 
 def test_group_grows_until_the_lists_fit_shared_memory():
-    # 148 jobs would get one CTA each, but 512 columns x ~780 rows x 6 B do not fit one CTA
-    jobs = [job(512, 512, 8) for _ in range(148)]
+    # 132 jobs would get one CTA each, but 512 columns x ~780 rows x 6 B do not fit one CTA
+    jobs = [job(512, 512, 8) for _ in range(132)]
     p = B.plan(jobs)
-    check_invariants(p, jobs, 148)
+    check_invariants(p, jobs, 132)
     assert p['ctas_per_problem'] > 1 and p['list_rows_smem'] >= (512 // p['ctas_per_problem']) * 3 // 2
     # a retry that asks for longer lists gets more spill rows
     longer = B.plan([dict(j, list_mul=8) for j in jobs])
@@ -84,7 +89,7 @@ def test_group_grows_until_the_lists_fit_shared_memory():
 def test_override_and_bad_arguments():
     p = B.plan([job(64, 64, 8)], group_override=7)
     assert p['ctas_per_problem'] == 7
-    assert B.plan([job(64, 64, 8)], group_override=1000)['ctas_per_problem'] == 148
+    assert B.plan([job(64, 64, 8)], group_override=1000)['ctas_per_problem'] == 132
     with pytest.raises(ValueError):
         B.plan([dict(n_in=0, n_out=4, nbits=4, digits=1)])
 
