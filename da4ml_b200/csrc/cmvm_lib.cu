@@ -6,6 +6,7 @@
 // candidates (and of all problems of a batch) are solved concurrently by one persistent kernel
 // launch per round.  All arithmetic of the path runs in the kernels of cmvm_kernels.cuh /
 // cmvm_decompose.cuh; nothing here falls back to the CPU.
+#include "dais_program.cuh"
 #include "host_solve.cuh"
 
 namespace da {
@@ -55,6 +56,141 @@ using namespace da;
 struct da4ml_pipeline {
     std::unique_ptr<PipelineImpl> impl;
 };
+
+// ---- DAIS interpreter engine ------------------------------------------------------------------------------------------
+// A loaded program: the validated host form plus its device copy (ops, level order, header arrays, table offsets and
+// tables), uploaded on first use on a device and kept until the handle is freed.
+struct da4ml_dais_program {
+    DaisProgramHost h;
+    int device = -1;
+    char *d_mem = nullptr;
+    size_t o_ops = 0, o_ord = 0, o_hdr = 0, o_toff = 0, o_tab = 0;
+    da4ml_dais_program() = default;
+    da4ml_dais_program(const da4ml_dais_program &) = delete;
+    ~da4ml_dais_program() {
+        if (d_mem)
+            cudaFree(d_mem);
+    }
+};
+
+namespace da {
+
+static void dais_upload(da4ml_dais_program &P, cudaStream_t st) {
+    int dev = 0;
+    CK(cudaGetDevice(&dev));
+    if (P.d_mem && P.device == dev)
+        return;
+    if (P.d_mem)
+        cudaFree(P.d_mem);
+    P.d_mem = nullptr;
+    const DaisProgramHost &h = P.h;
+    Carver c;
+    P.o_ops = c.take(sizeof(DaisOp) * h.ops.size());
+    P.o_ord = c.take(sizeof(int) * h.order.size());
+    P.o_hdr = c.take(sizeof(int32_t) * h.header.size());
+    P.o_toff = c.take(sizeof(long long) * h.table_off.size());
+    P.o_tab = c.take(sizeof(int32_t) * h.tables.size());
+    CK(cudaMalloc(&P.d_mem, std::max<size_t>(c.off, 256)));
+    P.device = dev;
+    auto up = [&](size_t off, const void *src, size_t bytes) {
+        if (bytes)
+            CK(cudaMemcpyAsync(P.d_mem + off, src, bytes, cudaMemcpyHostToDevice, st));
+    };
+    up(P.o_ops, h.ops.data(), sizeof(DaisOp) * h.ops.size());
+    up(P.o_ord, h.order.data(), sizeof(int) * h.order.size());
+    up(P.o_hdr, h.header.data(), sizeof(int32_t) * h.header.size());
+    up(P.o_toff, h.table_off.data(), sizeof(long long) * h.table_off.size());
+    up(P.o_tab, h.tables.data(), sizeof(int32_t) * h.tables.size());
+}
+
+// Run a program on n_samples rows on stream st.  Samples are processed in chunks that keep the [n_ops][S] int64 buffer
+// around 1 GB; with device_ptrs the inputs / outputs are read and written in place, otherwise they are staged through
+// device buffers.  A lookup out of range stops the run after its chunk with the reference's message for the first failing
+// (sample, op).
+//
+// Every run shares one scratch buffer, and a run on device pointers without lookups returns before its kernels finish.
+// Runs are therefore put in one order on the device whatever streams they come on: each run's stream first waits for the
+// event the previous run recorded after its last use of the scratch, and records it again after its own.  (A newly
+// uploaded program copy is written on the run's stream ahead of its kernels, so it is covered too.)
+static void dais_execute(da4ml_dais_program &P, const double *inputs, int64_t n_samples, double *outputs, bool device_ptrs, cudaStream_t st) {
+    if (n_samples == 0)
+        return;
+    init_device();
+    static cudaEvent_t scratch_free = nullptr; // recorded after the last run's final use of `work`
+    static int scratch_dev = -1;
+    if (scratch_dev != g_device) { // (a device change dropped every cached buffer, synchronising with the old device)
+        if (scratch_free)
+            cudaEventDestroy(scratch_free);
+        scratch_free = nullptr;
+        CK(cudaEventCreateWithFlags(&scratch_free, cudaEventDisableTiming));
+        CK(cudaEventRecord(scratch_free, st));
+        scratch_dev = g_device;
+    }
+    CK(cudaStreamWaitEvent(st, scratch_free, 0));
+    dais_upload(P, st);
+    const DaisProgramHost &h = P.h;
+    const int n_in = h.n_in, n_out = h.n_out, n_ops = h.n_ops;
+    const long long S_max = std::max<long long>(256, (1LL << 27) / std::max(1, n_ops));
+    const long long S = std::min<long long>(n_samples, S_max);
+    static DevBuf work;
+    Carver c;
+    const size_t o_in = c.take(device_ptrs ? 0 : sizeof(double) * S * n_in), o_out = c.take(device_ptrs ? 0 : sizeof(double) * S * n_out),
+                 o_buf = c.take(sizeof(long long) * S * n_ops), o_err = c.take(sizeof(unsigned long long));
+    if (c.off > work.cap)
+        CK(cudaEventSynchronize(scratch_free)); // the old buffer is freed: no earlier run may still be using it
+    work.ensure(c.off, false);
+    char *b = (char *)work.p;
+    const DaisOp *d_ops = (const DaisOp *)(P.d_mem + P.o_ops);
+    const int *d_ord = (const int *)(P.d_mem + P.o_ord), *d_hdr = (const int *)(P.d_mem + P.o_hdr);
+    const int *d_inp_shifts = d_hdr, *d_out_idxs = d_hdr + n_in, *d_out_shifts = d_out_idxs + n_out, *d_out_negs = d_out_shifts + n_out;
+    long long *d_buf = (long long *)(b + o_buf);
+    unsigned long long *d_err = (unsigned long long *)(b + o_err);
+    for (int64_t s0 = 0; s0 < n_samples; s0 += S) {
+        const long long Sc = std::min<long long>(S, n_samples - s0);
+        const double *d_in = device_ptrs ? inputs + s0 * n_in : (const double *)(b + o_in);
+        double *d_out = device_ptrs ? outputs + s0 * n_out : (double *)(b + o_out);
+        if (!device_ptrs && n_in)
+            CK(cudaMemcpyAsync(b + o_in, inputs + s0 * n_in, sizeof(double) * Sc * n_in, cudaMemcpyHostToDevice, st));
+        if (h.has_lookup)
+            CK(cudaMemsetAsync(d_err, 0xff, sizeof(unsigned long long), st));
+        for (int l = 0; l < h.n_levels; ++l) {
+            const int n_l = h.lvl_begin[l + 1] - h.lvl_begin[l];
+            const long long threads = (long long)n_l * Sc;
+            auto *kernel = h.lvl_adder[l] ? dais_level_kernel<true> : dais_level_kernel<false>;
+            kernel<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(
+                d_ops, d_ord + h.lvl_begin[l], n_l, d_inp_shifts, d_in, n_in, Sc, d_buf, (const int32_t *)(P.d_mem + P.o_tab), (const long long *)(P.d_mem + P.o_toff), d_err
+            );
+        }
+        if (n_out) {
+            const long long threads = (long long)n_out * Sc;
+            dais_output_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(d_ops, d_out_idxs, d_out_shifts, d_out_negs, n_out, Sc, d_buf, d_out);
+        }
+        CK(cudaGetLastError());
+        if (!device_ptrs && n_out)
+            CK(cudaMemcpyAsync(outputs + s0 * n_out, d_out, sizeof(double) * Sc * n_out, cudaMemcpyDeviceToHost, st));
+        if (h.has_lookup) {
+            unsigned long long key = 0;
+            CK(cudaMemcpyAsync(&key, d_err, sizeof(key), cudaMemcpyDeviceToHost, st));
+            CK(cudaEventRecord(scratch_free, st));
+            CK(cudaStreamSynchronize(st));
+            if (key != ~0ull) {
+                const long long s = (long long)(key >> 32);
+                const int i = (int)(key & 0xffffffffu);
+                long long v0 = 0;
+                CK(cudaMemcpyAsync(&v0, d_buf + (long long)h.ops[i].id0 * Sc + s, sizeof(v0), cudaMemcpyDeviceToHost, st));
+                CK(cudaStreamSynchronize(st));
+                throw ApiError(DA4ML_E_RUNTIME, dais_lookup_error(h, i, v0));
+            }
+        }
+        else {
+            CK(cudaEventRecord(scratch_free, st));
+            if (!device_ptrs)
+                CK(cudaStreamSynchronize(st));
+        }
+    }
+}
+
+} // namespace da
 
 template <class F> static int guarded(F &&f) {
     try {
@@ -449,7 +585,49 @@ int da4ml_cmvm_kernel_decompose(const float *kernel, int64_t n_in, int64_t n_out
     });
 }
 
-// ---- DAIS program replay (reference dais/bindings.cc `run_interp`), opcodes -1/0/1 -------------------------------
+// ---- DAIS interpreter (reference dais/bindings.cc `run_interp`) ------------------------------------------------------
+int da4ml_dais_program_load(const int32_t *words, int64_t n_words, da4ml_dais_program_t **out) {
+    return guarded([&] {
+        if (!out)
+            throw ApiError(DA4ML_E_INVALID, "invalid argument");
+        auto p = std::make_unique<da4ml_dais_program>();
+        dais_parse(words, n_words, p->h);
+        dais_validate(p->h);
+        dais_levelise(p->h);
+        *out = p.release();
+    });
+}
+
+int da4ml_dais_program_info(const da4ml_dais_program_t *p, int64_t info[6]) {
+    if (!p || !info)
+        return DA4ML_E_INVALID;
+    info[0] = p->h.n_in;
+    info[1] = p->h.n_out;
+    info[2] = p->h.n_ops;
+    info[3] = p->h.n_tables;
+    info[4] = p->h.n_levels;
+    info[5] = p->h.max_width;
+    return DA4ML_OK;
+}
+
+int da4ml_dais_program_run_stream(da4ml_dais_program_t *p, const double *inputs, int64_t n_samples, double *outputs, int device_ptrs, void *stream) {
+    return guarded([&] {
+        if (!p || n_samples < 0 || (n_samples > 0 && ((!inputs && p->h.n_in) || (!outputs && p->h.n_out))))
+            throw ApiError(DA4ML_E_INVALID, "invalid argument");
+        dais_execute(*p, inputs, n_samples, outputs, device_ptrs != 0, (cudaStream_t)stream);
+    });
+}
+
+int da4ml_dais_program_run(da4ml_dais_program_t *p, const double *inputs, int64_t n_samples, double *outputs, int device_ptrs) {
+    return da4ml_dais_program_run_stream(p, inputs, n_samples, outputs, device_ptrs, g_stream);
+}
+
+void da4ml_dais_program_free(da4ml_dais_program_t *p) {
+    std::lock_guard<std::mutex> lock(g_mutex);
+    delete p;
+}
+
+// Adder-graph programs only (opcodes -1/0/1, no tables): the checks and messages of the CMVM path, then the engine above.
 int da4ml_dais_run(const int32_t *program, int64_t n_words, const double *inputs, int64_t n_samples, double *outputs) {
     return guarded([&] {
         if (!program || n_words < 6 || !inputs || !outputs || n_samples < 0)
@@ -463,23 +641,10 @@ int da4ml_dais_run(const int32_t *program, int64_t n_words, const double *inputs
             throw ApiError(DA4ML_E_RUNTIME, "Binary data size mismatch (lookup tables are not produced by the CMVM path)");
         if (n_samples == 0)
             return;
-        init_device();
-        const int32_t *inp_shifts = program + 6, *out_idxs = inp_shifts + n_in, *out_shifts = out_idxs + n_out, *out_negs = out_shifts + n_out;
-        const DaisOp *hops = reinterpret_cast<const DaisOp *>(out_negs + n_out);
-        for (int i = 0; i < n_out; ++i) // (the reference interpreter indexes its buffer unchecked; a foreign file must not fault the device)
-            if (out_idxs[i] < -1 || out_idxs[i] >= n_ops)
-                throw ApiError(DA4ML_E_RUNTIME, "output index out of range at output " + std::to_string(i));
-        for (int i = 0; i < n_in; ++i)
-            if (inp_shifts[i] < -1023 || inp_shifts[i] > 1023)
-                throw ApiError(DA4ML_E_RUNTIME, "input shift out of range at input " + std::to_string(i));
-        for (int i = 0; i < n_out; ++i)
-            if (out_shifts[i] < -1023 || out_shifts[i] > 1023)
-                throw ApiError(DA4ML_E_RUNTIME, "output shift out of range at output " + std::to_string(i));
-        // causality + supported opcodes (DAISInterpreter::validate), levels
-        std::vector<int> level(n_ops, 0);
-        int n_levels = 1;
+        da4ml_dais_program prog;
+        dais_parse(program, n_words, prog.h); // (index and shift ranges of the header arrays)
         for (int i = 0; i < n_ops; ++i) {
-            const DaisOp &op = hops[i];
+            const DaisOp &op = prog.h.ops[i];
             if (op.opcode == -1) {
                 if (op.id0 < 0 || op.id0 >= n_in)
                     throw ApiError(DA4ML_E_RUNTIME, "input index out of range at operation " + std::to_string(i));
@@ -489,48 +654,9 @@ int da4ml_dais_run(const int32_t *program, int64_t n_words, const double *inputs
                 throw ApiError(DA4ML_E_RUNTIME, "Unknown opcode: " + std::to_string(op.opcode) + " at index " + std::to_string(i) + " (only adder graphs are replayed on this path)");
             if (op.id0 < 0 || op.id0 >= i || op.id1 < 0 || op.id1 >= i)
                 throw ApiError(DA4ML_E_RUNTIME, "Operation " + std::to_string(i) + " violating causality");
-            level[i] = 1 + std::max(level[op.id0], level[op.id1]);
-            n_levels = std::max(n_levels, level[i] + 1);
         }
-        std::vector<int> lvl_begin(n_levels + 1, 0), order(n_ops);
-        for (int i = 0; i < n_ops; ++i)
-            lvl_begin[level[i] + 1]++;
-        for (int l = 0; l < n_levels; ++l)
-            lvl_begin[l + 1] += lvl_begin[l];
-        {
-            std::vector<int> fill(lvl_begin.begin(), lvl_begin.end() - 1);
-            for (int i = 0; i < n_ops; ++i)
-                order[fill[level[i]]++] = i;
-        }
-        // samples per chunk: keep the [n_ops][S] int64 buffer around 1 GB
-        const long long S_max = std::max<long long>(256, (1LL << 27) / std::max(1, n_ops));
-        const long long S = std::min<long long>(n_samples, S_max);
-        static DevBuf buf;
-        Carver c;
-        size_t o_ops = c.take(sizeof(DaisOp) * n_ops), o_ord = c.take(sizeof(int) * n_ops), o_hdr = c.take(sizeof(int) * (n_in + 3 * n_out)),
-               o_in = c.take(sizeof(double) * S * n_in), o_out = c.take(sizeof(double) * S * n_out), o_buf = c.take(sizeof(long long) * S * n_ops);
-        buf.ensure(c.off, false);
-        char *b = (char *)buf.p;
-        CK(cudaMemcpyAsync(b + o_ops, hops, sizeof(DaisOp) * n_ops, cudaMemcpyHostToDevice, g_stream));
-        CK(cudaMemcpyAsync(b + o_ord, order.data(), sizeof(int) * n_ops, cudaMemcpyHostToDevice, g_stream));
-        CK(cudaMemcpyAsync(b + o_hdr, inp_shifts, sizeof(int) * (n_in + 3 * n_out), cudaMemcpyHostToDevice, g_stream));
-        const int *d_inp_shifts = (const int *)(b + o_hdr), *d_out_idxs = d_inp_shifts + n_in, *d_out_shifts = d_out_idxs + n_out, *d_out_negs = d_out_shifts + n_out;
-        for (int64_t s0 = 0; s0 < n_samples; s0 += S) {
-            const long long Sc = std::min<long long>(S, n_samples - s0);
-            CK(cudaMemcpyAsync(b + o_in, inputs + s0 * n_in, sizeof(double) * Sc * n_in, cudaMemcpyHostToDevice, g_stream));
-            for (int l = 0; l < n_levels; ++l) {
-                const int n_l = lvl_begin[l + 1] - lvl_begin[l];
-                if (!n_l)
-                    continue;
-                const long long threads = (long long)n_l * Sc;
-                dais_level_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, g_stream>>>((const DaisOp *)(b + o_ops), (const int *)(b + o_ord) + lvl_begin[l], n_l, d_inp_shifts, (const double *)(b + o_in), n_in, Sc, (long long *)(b + o_buf));
-            }
-            const long long threads = (long long)n_out * Sc;
-            dais_output_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, g_stream>>>((const DaisOp *)(b + o_ops), d_out_idxs, d_out_shifts, d_out_negs, n_out, Sc, (const long long *)(b + o_buf), (double *)(b + o_out));
-            CK(cudaGetLastError());
-            CK(cudaMemcpyAsync(outputs + s0 * n_out, b + o_out, sizeof(double) * Sc * n_out, cudaMemcpyDeviceToHost, g_stream));
-            CK(cudaStreamSynchronize(g_stream));
-        }
+        dais_levelise(prog.h);
+        dais_execute(prog, inputs, n_samples, outputs, false, g_stream);
     });
 }
 

@@ -130,11 +130,34 @@ int64_t da4ml_pipeline_launches(const da4ml_pipeline_t *p);
  * algorithmic_bytes (all solve_single jobs of the call, exact in accounting mode), 0, 0, 0}. */
 int da4ml_pipeline_profile(const da4ml_pipeline_t *p, double out[8]);
 
-/* ---- DAIS replay (SURVEY 8f N2) -------------------------------------------------------------------
- * Replaces `run_interp` of the reference's second native module (dais/bindings.cc:32-110 -> DAISInterpreter.cc) for
- * the programs the CMVM path produces (opcodes -1, 0, 1; no lookup tables): `program` = int32 words of
- * CombLogic.to_binary (types.py:500-541), inputs [n_samples, n_in] float64, outputs [n_samples, n_out] float64.
- * Bit-exact int64 fixed-point semantics of the reference interpreter. */
+/* ---- DAIS interpreter (SURVEY 8f N2) ----------------------------------------------------------------
+ * Replaces `run_interp` of the reference's second native module (dais/bindings.cc:30-131 -> DAISInterpreter.cc) for
+ * every DAIS program: all opcodes of DAISInterpreter::exec_ops and lookup tables.  Programs are the int32 words of
+ * CombLogic.to_binary (types.py:500-541); inputs [n_samples, n_in] float64, outputs [n_samples, n_out] float64, both
+ * row-major.  Bit-exact int64 fixed-point semantics of the reference interpreter's compiled code. */
+typedef struct da4ml_dais_program da4ml_dais_program_t; /* opaque loaded program */
+
+/* Parse and validate a program on the host (no device call): size, version and table block, causality, opcodes, operand
+ * ids, table indices, mux shift configurations, bit-op kinds.  Errors return DA4ML_E_RUNTIME with the reference's
+ * wording where it has one.  Free with da4ml_dais_program_free. */
+int da4ml_dais_program_load(const int32_t *words, int64_t n_words, da4ml_dais_program_t **out);
+/* info: {n_in, n_out, n_ops, n_tables, n_levels, max op width} */
+int da4ml_dais_program_info(const da4ml_dais_program_t *p, int64_t info[6]);
+/* Run on n_samples rows on the stream set with da4ml_cmvm_set_stream.  device_ptrs = 1: inputs / outputs are device
+ * pointers, used in place, and the call returns without waiting unless the program has lookups.  Runs of any programs on
+ * any streams are executed one after the other on the device (they share the library's scratch buffer), each ordered
+ * after the work already queued on its own stream.  A lookup index out of range fails with the reference's message for
+ * the first failing sample (lowest sample, then lowest op); outputs of the chunk that failed and of later chunks are
+ * then unspecified. */
+int da4ml_dais_program_run(da4ml_dais_program_t *p, const double *inputs, int64_t n_samples, double *outputs, int device_ptrs);
+/* Same, on the given stream (cudaStream_t as void*) instead of the library's stream, which stays as it is. */
+int da4ml_dais_program_run_stream(
+    da4ml_dais_program_t *p, const double *inputs, int64_t n_samples, double *outputs, int device_ptrs, void *cuda_stream
+);
+void da4ml_dais_program_free(da4ml_dais_program_t *p);
+
+/* The programs the CMVM path produces only (opcodes -1, 0, 1; no lookup tables), host arrays; any other program is
+ * refused.  Same engine as da4ml_dais_program_run. */
 int da4ml_dais_run(const int32_t *program, int64_t n_words, const double *inputs, int64_t n_samples, double *outputs);
 
 /* ---- helpers exported by the reference module -------------------------------------------------- */
