@@ -62,6 +62,8 @@ _L.da4ml_dais_program_load.argtypes = [_i32p, C.c_int64, C.POINTER(_vp)]
 _L.da4ml_dais_program_info.argtypes = [_vp, _i64p]
 _L.da4ml_dais_program_run.argtypes = [_vp, _vp, C.c_int64, _vp, C.c_int]
 _L.da4ml_dais_program_run_stream.argtypes = [_vp, _vp, C.c_int64, _vp, C.c_int, _vp]
+_L.da4ml_dais_program_profile.argtypes = [_vp, _vp, C.c_int64, C.c_int, _vp, _vp]
+_L.da4ml_dais_program_dump.argtypes = [_vp, _vp, C.c_int64, _vp, C.c_int64, _vp, C.c_int, _vp]
 _L.da4ml_dais_program_free.argtypes = [_vp]
 _L.da4ml_dais_program_free.restype = None
 _L.da4ml_cmvm_get_lsb_loc.argtypes = [C.c_float]
@@ -77,7 +79,7 @@ EXPORTED_SYMBOLS = [
     'da4ml_cmvm_csd_decompose', 'da4ml_cmvm_int_arr_to_csd', 'da4ml_cmvm_kernel_decompose',
     'da4ml_cmvm_get_lsb_loc', 'da4ml_cmvm_iceil_log2', 'da4ml_cmvm_cost_add', 'da4ml_dais_run',
     'da4ml_dais_program_load', 'da4ml_dais_program_info', 'da4ml_dais_program_run', 'da4ml_dais_program_run_stream',
-    'da4ml_dais_program_free',
+    'da4ml_dais_program_free', 'da4ml_dais_program_profile', 'da4ml_dais_program_dump',
 ]  # fmt: skip
 
 COUNTER_NAMES = ['status', 'n_ops', 'T', 'sum_F', 'sum_R', 'F0', 'R0', 'D_final', 'F_max', 'compactions', 'D0', 'n_bits', 'group_ctas',

@@ -103,18 +103,38 @@ static void dais_upload(da4ml_dais_program &P, cudaStream_t st) {
     up(P.o_tab, h.tables.data(), sizeof(int32_t) * h.tables.size());
 }
 
+// What a pass over the samples produces from each chunk's buffer after its last level: the program's outputs (run), the
+// codes of selected ops (dump), or per-op statistics of every op's codes (profile).
+enum class DaisPass { run, dump, profile };
+struct DaisRequest {
+    DaisPass pass = DaisPass::run;
+    const int32_t *sel = nullptr; // dump: op ids [n_sel], host memory
+    int64_t n_sel = 0;
+    long long *stats = nullptr;   // profile: [n_ops][3] int64 host = {min, max, bitwise OR}
+};
+
 // Run a program on n_samples rows on stream st.  Samples are processed in chunks that keep the [n_ops][S] int64 buffer
 // around 1 GB; with device_ptrs the inputs / outputs are read and written in place, otherwise they are staged through
-// device buffers.  A lookup out of range stops the run after its chunk with the reference's message for the first failing
-// (sample, op).
+// device buffers.  `outputs` holds 8-byte rows of n_out doubles (run) or n_sel int64 codes (dump); a profile has none and
+// copies its statistics to the host once, after the last chunk.  A lookup out of range stops the run after its chunk
+// with the reference's message for the first failing (sample, op).
 //
 // Every run shares one scratch buffer, and a run on device pointers without lookups returns before its kernels finish.
 // Runs are therefore put in one order on the device whatever streams they come on: each run's stream first waits for the
 // event the previous run recorded after its last use of the scratch, and records it again after its own.  (A newly
-// uploaded program copy is written on the run's stream ahead of its kernels, so it is covered too.)
-static void dais_execute(da4ml_dais_program &P, const double *inputs, int64_t n_samples, double *outputs, bool device_ptrs, cudaStream_t st) {
-    if (n_samples == 0)
+// uploaded program copy is written on the run's stream ahead of its kernels, so it is covered too, as are the selected op
+// ids and the statistics accumulators, which live in the scratch.)
+static void dais_execute(da4ml_dais_program &P, const double *inputs, int64_t n_samples, void *outputs, bool device_ptrs, cudaStream_t st,
+                         const DaisRequest &req = DaisRequest()) {
+    const DaisPass pass = req.pass;
+    if (n_samples == 0) {
+        for (int i = 0; pass == DaisPass::profile && i < P.h.n_ops; ++i) {
+            req.stats[3LL * i] = LLONG_MAX;
+            req.stats[3LL * i + 1] = LLONG_MIN;
+            req.stats[3LL * i + 2] = 0;
+        }
         return;
+    }
     init_device();
     static cudaEvent_t scratch_free = nullptr; // recorded after the last run's final use of `work`
     static int scratch_dev = -1;
@@ -130,12 +150,16 @@ static void dais_execute(da4ml_dais_program &P, const double *inputs, int64_t n_
     dais_upload(P, st);
     const DaisProgramHost &h = P.h;
     const int n_in = h.n_in, n_out = h.n_out, n_ops = h.n_ops;
-    const long long S_max = std::max<long long>(256, (1LL << 27) / std::max(1, n_ops));
+    // columns of an output row (8 bytes each); a dump with more columns than ops takes smaller chunks, so its staged
+    // output stays the size of the buffer
+    const long long n_cols = pass == DaisPass::run ? n_out : pass == DaisPass::dump ? req.n_sel : 0;
+    const long long S_max = std::max<long long>(256, (1LL << 27) / std::max<long long>({1, n_ops, pass == DaisPass::dump ? n_cols : 0}));
     const long long S = std::min<long long>(n_samples, S_max);
     static DevBuf work;
     Carver c;
-    const size_t o_in = c.take(device_ptrs ? 0 : sizeof(double) * S * n_in), o_out = c.take(device_ptrs ? 0 : sizeof(double) * S * n_out),
-                 o_buf = c.take(sizeof(long long) * S * n_ops), o_err = c.take(sizeof(unsigned long long));
+    const size_t o_in = c.take(device_ptrs ? 0 : sizeof(double) * S * n_in), o_out = c.take(device_ptrs ? 0 : sizeof(double) * S * n_cols),
+                 o_buf = c.take(sizeof(long long) * S * n_ops), o_err = c.take(sizeof(unsigned long long)),
+                 o_sel = c.take(pass == DaisPass::dump ? sizeof(int32_t) * req.n_sel : 0), o_stats = c.take(pass == DaisPass::profile ? sizeof(long long) * 3 * n_ops : 0);
     if (c.off > work.cap)
         CK(cudaEventSynchronize(scratch_free)); // the old buffer is freed: no earlier run may still be using it
     work.ensure(c.off, false);
@@ -145,10 +169,17 @@ static void dais_execute(da4ml_dais_program &P, const double *inputs, int64_t n_
     const int *d_inp_shifts = d_hdr, *d_out_idxs = d_hdr + n_in, *d_out_shifts = d_out_idxs + n_out, *d_out_negs = d_out_shifts + n_out;
     long long *d_buf = (long long *)(b + o_buf);
     unsigned long long *d_err = (unsigned long long *)(b + o_err);
+    const int *d_sel = (const int *)(b + o_sel);
+    long long *d_stats = (long long *)(b + o_stats);
+    std::vector<long long> stats(pass == DaisPass::profile ? 3 * (size_t)n_ops : 0);
+    if (pass == DaisPass::dump && req.n_sel)
+        CK(cudaMemcpyAsync(b + o_sel, req.sel, sizeof(int32_t) * req.n_sel, cudaMemcpyHostToDevice, st));
+    if (pass == DaisPass::profile && n_ops)
+        dais_stats_init_kernel<<<(n_ops + 255) / 256, 256, 0, st>>>(d_stats, n_ops);
     for (int64_t s0 = 0; s0 < n_samples; s0 += S) {
         const long long Sc = std::min<long long>(S, n_samples - s0);
         const double *d_in = device_ptrs ? inputs + s0 * n_in : (const double *)(b + o_in);
-        double *d_out = device_ptrs ? outputs + s0 * n_out : (double *)(b + o_out);
+        char *d_out = device_ptrs ? (char *)outputs + 8 * s0 * n_cols : b + o_out;
         if (!device_ptrs && n_in)
             CK(cudaMemcpyAsync(b + o_in, inputs + s0 * n_in, sizeof(double) * Sc * n_in, cudaMemcpyHostToDevice, st));
         if (h.has_lookup)
@@ -161,13 +192,23 @@ static void dais_execute(da4ml_dais_program &P, const double *inputs, int64_t n_
                 d_ops, d_ord + h.lvl_begin[l], n_l, d_inp_shifts, d_in, n_in, Sc, d_buf, (const int32_t *)(P.d_mem + P.o_tab), (const long long *)(P.d_mem + P.o_toff), d_err
             );
         }
-        if (n_out) {
+        if (pass == DaisPass::run && n_out) {
             const long long threads = (long long)n_out * Sc;
-            dais_output_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(d_ops, d_out_idxs, d_out_shifts, d_out_negs, n_out, Sc, d_buf, d_out);
+            dais_output_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(d_ops, d_out_idxs, d_out_shifts, d_out_negs, n_out, Sc, d_buf, (double *)d_out);
+        }
+        if (pass == DaisPass::dump && n_cols) {
+            const long long tiles = (n_cols + 31) / 32;
+            dais_dump_kernel<<<dim3((unsigned)((Sc + 31) / 32), (unsigned)std::min<long long>(tiles, 65535)), dim3(32, 8), 0, st>>>(d_buf, Sc, d_sel, n_cols, (long long *)d_out);
+        }
+        if (pass == DaisPass::profile && n_ops) {
+            const long long per_block = (long long)kDaisStatsThreads * kDaisStatsPerThread;
+            dais_stats_kernel<<<dim3((unsigned)n_ops, (unsigned)std::min<long long>((Sc + per_block - 1) / per_block, 65535)), kDaisStatsThreads, 0, st>>>(d_buf, Sc, d_stats);
+            if (s0 + Sc == n_samples) // the accumulators leave the scratch before the event below frees it
+                CK(cudaMemcpyAsync(stats.data(), d_stats, sizeof(long long) * 3 * n_ops, cudaMemcpyDeviceToHost, st));
         }
         CK(cudaGetLastError());
-        if (!device_ptrs && n_out)
-            CK(cudaMemcpyAsync(outputs + s0 * n_out, d_out, sizeof(double) * Sc * n_out, cudaMemcpyDeviceToHost, st));
+        if (!device_ptrs && n_cols)
+            CK(cudaMemcpyAsync((char *)outputs + 8 * s0 * n_cols, d_out, 8 * Sc * n_cols, cudaMemcpyDeviceToHost, st));
         if (h.has_lookup) {
             unsigned long long key = 0;
             CK(cudaMemcpyAsync(&key, d_err, sizeof(key), cudaMemcpyDeviceToHost, st));
@@ -184,10 +225,12 @@ static void dais_execute(da4ml_dais_program &P, const double *inputs, int64_t n_
         }
         else {
             CK(cudaEventRecord(scratch_free, st));
-            if (!device_ptrs)
+            if (!device_ptrs || (pass == DaisPass::profile && s0 + Sc == n_samples))
                 CK(cudaStreamSynchronize(st));
         }
     }
+    if (pass == DaisPass::profile) // (only once every chunk passed its lookup check)
+        std::copy(stats.begin(), stats.end(), req.stats);
 }
 
 } // namespace da
@@ -620,6 +663,50 @@ int da4ml_dais_program_run_stream(da4ml_dais_program_t *p, const double *inputs,
 
 int da4ml_dais_program_run(da4ml_dais_program_t *p, const double *inputs, int64_t n_samples, double *outputs, int device_ptrs) {
     return da4ml_dais_program_run_stream(p, inputs, n_samples, outputs, device_ptrs, g_stream);
+}
+
+int da4ml_dais_program_profile(da4ml_dais_program_t *p, const double *inputs, int64_t n_samples, int device_ptrs, void *cuda_stream, int64_t *stats) {
+    return guarded([&] {
+        if (!p)
+            throw ApiError(DA4ML_E_INVALID, "profile: the program handle is null");
+        if (n_samples < 0)
+            throw ApiError(DA4ML_E_INVALID, "profile: n_samples is negative (" + std::to_string(n_samples) + ")");
+        if (n_samples > 0 && p->h.n_in && !inputs)
+            throw ApiError(DA4ML_E_INVALID, "profile: inputs is null");
+        if (p->h.n_ops && !stats)
+            throw ApiError(DA4ML_E_INVALID, "profile: stats is null");
+        DaisRequest req;
+        req.pass = DaisPass::profile;
+        req.stats = (long long *)stats;
+        dais_execute(*p, inputs, n_samples, nullptr, device_ptrs != 0, (cudaStream_t)cuda_stream, req);
+    });
+}
+
+int da4ml_dais_program_dump(da4ml_dais_program_t *p, const double *inputs, int64_t n_samples, const int32_t *op_ids, int64_t n_sel, int64_t *values, int device_ptrs,
+                            void *cuda_stream) {
+    return guarded([&] {
+        if (!p)
+            throw ApiError(DA4ML_E_INVALID, "dump: the program handle is null");
+        if (n_samples < 0)
+            throw ApiError(DA4ML_E_INVALID, "dump: n_samples is negative (" + std::to_string(n_samples) + ")");
+        if (n_sel < 0)
+            throw ApiError(DA4ML_E_INVALID, "dump: n_sel is negative (" + std::to_string(n_sel) + ")");
+        if (n_sel > 0 && !op_ids)
+            throw ApiError(DA4ML_E_INVALID, "dump: op_ids is null");
+        for (int64_t k = 0; k < n_sel; ++k)
+            if (op_ids[k] < 0 || op_ids[k] >= p->h.n_ops)
+                throw ApiError(DA4ML_E_INVALID, "dump: op id " + std::to_string(op_ids[k]) + " at position " + std::to_string(k) + " is out of range [0, " +
+                                                    std::to_string(p->h.n_ops) + ")");
+        if (n_samples > 0 && p->h.n_in && !inputs)
+            throw ApiError(DA4ML_E_INVALID, "dump: inputs is null");
+        if (n_samples > 0 && n_sel > 0 && !values)
+            throw ApiError(DA4ML_E_INVALID, "dump: values is null");
+        DaisRequest req;
+        req.pass = DaisPass::dump;
+        req.sel = op_ids;
+        req.n_sel = n_sel;
+        dais_execute(*p, inputs, n_samples, values, device_ptrs != 0, (cudaStream_t)cuda_stream, req);
+    });
 }
 
 void da4ml_dais_program_free(da4ml_dais_program_t *p) {

@@ -264,6 +264,99 @@ __global__ void __launch_bounds__(256) dais_output_kernel(
     const int idx = out_idxs[o];
     outputs[s * n_out + o] = idx >= 0 ? dais_output(buffer[(long long)idx * S + s], out_negs[o], out_shifts[o], ops[idx].fractionals) : 0.0;
 }
+
+// ---- op profiling: per-op statistics and dumps of the codes in the buffer, after a chunk's last level ----------------
+// stats: [n_ops][3] int64 = {min, max, bitwise OR} of each op's codes, folded over every chunk of a call.
+__global__ void dais_stats_init_kernel(long long *stats, int n_ops) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_ops)
+        return;
+    stats[3LL * i] = LLONG_MAX;
+    stats[3LL * i + 1] = LLONG_MIN;
+    stats[3LL * i + 2] = 0;
+}
+
+// grid (n_ops, sample blocks): each block reduces a slice of one op's row (contiguous, so the loads are coalesced) with
+// warp shuffles and shared memory, then folds it into the op's accumulators with one atomic per statistic.
+constexpr int kDaisStatsThreads = 256, kDaisStatsPerThread = 8;
+__global__ void __launch_bounds__(kDaisStatsThreads) dais_stats_kernel(const long long *__restrict__ buffer, long long S, long long *stats) {
+    const int i = blockIdx.x;
+    const long long *row = buffer + (long long)i * S;
+    long long mn = LLONG_MAX, mx = LLONG_MIN;
+    unsigned long long bits = 0;
+    constexpr long long kSpan = (long long)kDaisStatsThreads * kDaisStatsPerThread; // samples per block and pass
+    for (long long s0 = (long long)blockIdx.y * kSpan + threadIdx.x; s0 < S; s0 += (long long)gridDim.y * kSpan) {
+        long long v[kDaisStatsPerThread]; // all loads issued before any is used
+#pragma unroll
+        for (int k = 0; k < kDaisStatsPerThread; ++k) {
+            const long long s = s0 + (long long)k * kDaisStatsThreads;
+            v[k] = s < S ? __ldg(row + s) : row[s0];
+        }
+#pragma unroll
+        for (int k = 0; k < kDaisStatsPerThread; ++k) {
+            mn = min(mn, v[k]);
+            mx = max(mx, v[k]);
+            bits |= (unsigned long long)v[k];
+        }
+    }
+    for (int off = 16; off > 0; off >>= 1) {
+        mn = min(mn, __shfl_xor_sync(0xffffffffu, mn, off));
+        mx = max(mx, __shfl_xor_sync(0xffffffffu, mx, off));
+        bits |= __shfl_xor_sync(0xffffffffu, bits, off);
+    }
+    __shared__ long long s_mn[kDaisStatsThreads / 32], s_mx[kDaisStatsThreads / 32];
+    __shared__ unsigned long long s_bits[kDaisStatsThreads / 32];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (lane == 0) {
+        s_mn[warp] = mn;
+        s_mx[warp] = mx;
+        s_bits[warp] = bits;
+    }
+    __syncthreads();
+    if (warp)
+        return;
+    const bool live = lane < kDaisStatsThreads / 32;
+    mn = live ? s_mn[lane] : LLONG_MAX;
+    mx = live ? s_mx[lane] : LLONG_MIN;
+    bits = live ? s_bits[lane] : 0;
+    for (int off = kDaisStatsThreads / 64; off > 0; off >>= 1) {
+        mn = min(mn, __shfl_xor_sync(0xffffffffu, mn, off));
+        mx = max(mx, __shfl_xor_sync(0xffffffffu, mx, off));
+        bits |= __shfl_xor_sync(0xffffffffu, bits, off);
+    }
+    if (lane == 0) {
+        long long *st = stats + 3LL * i;
+        atomicMin(st, mn);
+        atomicMax(st + 1, mx);
+        atomicOr((unsigned long long *)(st + 2), bits);
+    }
+}
+
+// values [S][n_sel] = codes of ops sel[0..n_sel) for the S samples of the chunk.  Block (32, 8), one 32-sample x 32-op
+// tile at a time through shared memory: the reads run along the buffer's rows (samples), the writes along the output's
+// rows (selected ops), so both are coalesced.  grid.x covers the samples, grid.y strides over the tiles of ops.
+__global__ void __launch_bounds__(256) dais_dump_kernel(
+    const long long *__restrict__ buffer, long long S, const int *__restrict__ sel, long long n_sel, long long *__restrict__ values
+) {
+    __shared__ long long tile[32][33]; // (+1 column: the transposed reads hit distinct banks)
+    const long long s0 = (long long)blockIdx.x * 32;
+    const long long n_tiles = (n_sel + 31) / 32;
+    for (long long jt = blockIdx.y; jt < n_tiles; jt += gridDim.y) {
+        const long long j0 = jt * 32;
+        for (int r = threadIdx.y; r < 32; r += 8) {
+            const long long j = j0 + r, s = s0 + threadIdx.x;
+            if (j < n_sel && s < S)
+                tile[r][threadIdx.x] = buffer[(long long)sel[j] * S + s];
+        }
+        __syncthreads();
+        for (int r = threadIdx.y; r < 32; r += 8) {
+            const long long j = j0 + threadIdx.x, s = s0 + r;
+            if (j < n_sel && s < S)
+                values[s * n_sel + j] = tile[threadIdx.x][r];
+        }
+        __syncthreads();
+    }
+}
 #endif
 
 } // namespace da

@@ -154,6 +154,18 @@ int da4ml_dais_program_run(da4ml_dais_program_t *p, const double *inputs, int64_
 int da4ml_dais_program_run_stream(
     da4ml_dais_program_t *p, const double *inputs, int64_t n_samples, double *outputs, int device_ptrs, void *cuda_stream
 );
+/* Profiling: an op's code is its int64 value in the interpreter (its real value is code * 2^-fractionals).  Both calls
+ * run the program as da4ml_dais_program_run_stream does, on the given stream, with the same ordering and lookup errors,
+ * and check their arguments on the host before any device call (DA4ML_E_INVALID). */
+/* Per-op statistics of the op codes over n_samples rows, on the given stream: stats [n_ops][3] int64 host =
+ * {min, max, bitwise OR}; identity {INT64_MAX, INT64_MIN, 0} for zero samples.  Synchronises.  On a lookup error the
+ * reference's message is returned and stats is not written. */
+int da4ml_dais_program_profile(da4ml_dais_program_t *p, const double *inputs, int64_t n_samples, int device_ptrs,
+                               void *cuda_stream, int64_t *stats);
+/* Codes of ops op_ids[0..n_sel) for every row: values [n_samples][n_sel] int64 (device pointer when device_ptrs).
+ * op_ids is host memory; ids may repeat.  Returns without waiting under the same conditions as a run. */
+int da4ml_dais_program_dump(da4ml_dais_program_t *p, const double *inputs, int64_t n_samples, const int32_t *op_ids,
+                            int64_t n_sel, int64_t *values, int device_ptrs, void *cuda_stream);
 void da4ml_dais_program_free(da4ml_dais_program_t *p);
 
 /* The programs the CMVM path produces only (opcodes -1, 0, 1; no lookup tables), host arrays; any other program is

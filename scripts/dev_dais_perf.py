@@ -1,11 +1,13 @@
 """Throughput of the DAIS interpreter (da4ml_b200.dais) on the GPU, with the hardware it ran on.
 
-  python scripts/dev_dais_perf.py [--samples N] [--parent-lib PATH] [--out FILE]
+  python scripts/dev_dais_perf.py [--samples N] [--ref-samples N] [--dump-samples N] [--parent-lib PATH] [--out FILE]
 
 Programs: the largest traced fixture (tests/golden/dais_programs.json.gz, ``traced_mlp``) and the stage-0 adder graph
 of a 256x256 int8 solve.  For each: samples/s of the device path (inputs and outputs resident, CUDA events around one
 call), and bytes moved per the buffer model (8 B per operand read plus 8 B per result write, per op and sample) over
-that time, against the H100 SXM data-sheet HBM bandwidth (3.35 TB/s).  The reference interpreter
+that time, against the H100 SXM data-sheet HBM bandwidth (3.35 TB/s).  In the same loop, alternated with the run:
+``DaisProgram.profile`` on the same inputs (its time and the ratio to the run), and for the traced MLP the all-ops
+``DaisProgram.dump`` of the first --dump-samples samples, in GB/s written.  The reference interpreter
 (oracle/_ref/libdais_ref.so) runs on all host cores in the same process, one thread per core over sample chunks as the
 reference's OpenMP loop does.  With --parent-lib (a libda4ml_b200_cmvm.so built from an earlier revision), the adder
 graph is also replayed by that library's da4ml_dais_run and this one's, alternated, timing the kernels with
@@ -49,25 +51,35 @@ def buffer_bytes(prog) -> float:
     return float(sum(8 * (reads.get(int(o), 1) + 1) for o in ops[:, 0]))
 
 
-def time_device(prog, x_np, reps=5):
+def time_device(prog, x_np, reps=5, dump_samples=0):
+    """Device seconds {call: [reps]} of a run, a profile and (dump_samples > 0) an all-ops dump of that many samples,
+    alternated; and the run's outputs."""
     import torch
 
     from da4ml_b200.dais import DaisProgram
 
     p = DaisProgram(prog)
     x = torch.from_numpy(x_np).cuda()
-    p(x[:1024])
+    calls = dict(run=lambda: p(x), profile=lambda: p.profile(x))
+    if dump_samples:
+        calls['dump'] = lambda: p.dump(x[:dump_samples])
+    for fn in calls.values():  # (uploads the program, grows the scratch)
+        fn()
     torch.cuda.synchronize()
-    ts = []
+    ts = {k: [] for k in calls}
     for _ in range(reps):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        y = p(x)
-        b.record()
-        torch.cuda.synchronize()
-        ts.append(a.elapsed_time(b) / 1e3)
+        for k, fn in calls.items():
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record()
+            out = fn()
+            b.record()
+            torch.cuda.synchronize()
+            ts[k].append(a.elapsed_time(b) / 1e3)
+            if k == 'run':
+                y = out
+            del out
     p.close()
-    return float(np.median(ts)), float(min(ts)), y
+    return ts, y
 
 
 def time_reference(prog, x, threads):
@@ -101,7 +113,8 @@ def kernel_seconds(fn):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--samples', type=int, default=1_000_000)
-    ap.add_argument('--ref-samples', type=int, default=200_000)
+    ap.add_argument('--ref-samples', type=int, default=200_000, help='0 skips the reference interpreter')
+    ap.add_argument('--dump-samples', type=int, default=100_000)
     ap.add_argument('--parent-lib', default='')
     ap.add_argument('--out', default='')
     a = ap.parse_args()
@@ -120,14 +133,21 @@ def main():
         ('traced_mlp', mlp, G.random_inputs(11, a.samples, int(mlp[2]))),
         ('adder_256x256_stage0', adder, np.random.default_rng(1).integers(-128, 128, size=(a.samples, 256)).astype(np.float64)),
     ):
-        med, best, y = time_device(prog, x)
+        ts, y = time_device(prog, x, dump_samples=min(a.dump_samples, a.samples) if name == 'traced_mlp' else 0)
+        med, best = float(np.median(ts['run'])), float(min(ts['run']))
         nb = buffer_bytes(prog) * a.samples
-        n_ref = min(a.ref_samples, a.samples)
-        t_ref, y_ref = time_reference(prog, x[:n_ref], res['host_cores'])
-        same = bool(np.array_equal(y[:n_ref].cpu().numpy().view(np.uint64), y_ref.view(np.uint64)))
         r = dict(n_ops=int(prog[4]), n_in=int(prog[2]), n_out=int(prog[3]), device_s_median=med, device_s_best=best, samples_per_s=a.samples / med,
-                 buffer_bytes=nb, buffer_tbs=nb / med / 1e12, hbm_fraction=nb / med / 1e12 / HBM_TBS, ref_samples=n_ref, ref_s=t_ref,
-                 ref_samples_per_s=n_ref / t_ref, ref_equal=same)  # fmt: skip
+                 buffer_bytes=nb, buffer_tbs=nb / med / 1e12, hbm_fraction=nb / med / 1e12 / HBM_TBS, run_s=ts['run'], profile_s=ts['profile'],
+                 profile_s_median=float(np.median(ts['profile'])), profile_over_run=float(np.median(ts['profile'])) / med)  # fmt: skip
+        if 'dump' in ts:
+            n_dump = min(a.dump_samples, a.samples)
+            t = float(np.median(ts['dump']))
+            r.update(dump_samples=n_dump, dump_s=ts['dump'], dump_s_median=t, dump_gbs_written=n_dump * int(prog[4]) * 8 / t / 1e9)
+        n_ref = min(a.ref_samples, a.samples)
+        if n_ref:
+            t_ref, y_ref = time_reference(prog, x[:n_ref], res['host_cores'])
+            same = bool(np.array_equal(y[:n_ref].cpu().numpy().view(np.uint64), y_ref.view(np.uint64)))
+            r.update(ref_samples=n_ref, ref_s=t_ref, ref_samples_per_s=n_ref / t_ref, ref_equal=same)
         res['programs'][name] = r
         print(name, json.dumps(r), flush=True)
     if a.parent_lib:
