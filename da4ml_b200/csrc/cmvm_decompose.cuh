@@ -2,7 +2,8 @@
 // (reference mat_decompose.cc:6-137; centring bit_decompose.hh:21-34).
 //
 //   center_kernel    power-of-two normalisation of columns then rows, augmented matrix [0 | centred]
-//   dist_kernel      all-pairs column distance = min(CSD weight(a-b), CSD weight(a+b)) summed over rows
+//   dist_kernel      all-pairs column distance = min(CSD weight(a-b), CSD weight(a+b)) summed over rows, each weight
+//                    at the CSD width of its whole array, as the reference counts it
 //   mst_build_kernel one CTA per delay-constraint candidate: Prim MST with the reference's first-minimum
 //                    tie-break, then the sequential construction of M0 (edge columns) and M1 (path matrix)
 #pragma once
@@ -40,17 +41,67 @@ __global__ void __launch_bounds__(256) center_kernel(const float *kernel, int n_
         aug[(size_t)i * n] = 0.0f;
 }
 
+// The reference decomposes the whole [n_in][n][n] array of differences, and that of sums, each with one CSD width taken
+// from its largest |int32| (mat_decompose.cc:81-84).  Every CTA first finds both maxima itself: one warp per row takes
+// the row's max and min, which bound every difference and sum of the row.  Only a row whose bounds leave the int32 range
+// (or that holds a NaN) is searched pair by pair, because its out-of-range values convert to INT32_MIN and take no part.
+__device__ __forceinline__ void row_csd_maxima(const float *row, int n, int lane, int &m0, int &m1) {
+    float hi = 0.0f, lo = 0.0f; // (column 0 is zero)
+    bool bad = false;
+    for (int a = lane; a < n; a += 32) {
+        const float v = row[a];
+        bad |= v != v;
+        hi = fmaxf(hi, v);
+        lo = fminf(lo, v);
+    }
+    for (int off = 16; off > 0; off >>= 1) {
+        hi = fmaxf(hi, __shfl_xor_sync(0xffffffffu, hi, off));
+        lo = fminf(lo, __shfl_xor_sync(0xffffffffu, lo, off));
+        bad |= __shfl_xor_sync(0xffffffffu, (int)bad, off) != 0;
+    }
+    const float d = fsub(hi, lo), s_hi = fadd(hi, hi), s_lo = fadd(lo, lo); // rounding is monotone: the extremes
+    if (!bad && d < 2147483648.0f && s_hi < 2147483648.0f && s_lo > -2147483648.0f) {
+        m0 = max(m0, csd_abs(trunc_i32(d)));
+        m1 = max(m1, max(csd_abs(trunc_i32(s_hi)), csd_abs(trunc_i32(s_lo))));
+        return;
+    }
+    for (int a = lane; a < n; a += 32)
+        for (int b = a; b < n; ++b) { // both are symmetric in (a, b)
+            m0 = max(m0, csd_abs(trunc_i32(fsub(row[a], row[b]))));
+            m1 = max(m1, csd_abs(trunc_i32(fadd(row[a], row[b]))));
+        }
+}
+
 // dist[a][b] (int32) and sign[a][b] (int8), n = n_out + 1 (mat_decompose.cc:73-93)
 __global__ void __launch_bounds__(256) dist_kernel(const float *aug, int n_in, int n, int *dist, int8_t *sign) {
-    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+#ifdef DA_CPU_SIM
+    DA_SHARED_VAR(int, s_max0);
+    DA_SHARED_VAR(int, s_max1);
+#else
+    __shared__ int s_max0, s_max1;
+#endif
+    const int tid = threadIdx.x, lane = tid & 31;
+    if (tid == 0) {
+        s_max0 = 0;
+        s_max1 = 0;
+    }
+    __syncthreads();
+    int m0 = 0, m1 = 0;
+    for (int i = tid >> 5; i < n_in; i += blockDim.x >> 5)
+        row_csd_maxima(aug + (size_t)i * n, n, lane, m0, m1);
+    atomicMax(&s_max0, m0);
+    atomicMax(&s_max1, m1);
+    __syncthreads();
+    const long long idx = (long long)blockIdx.x * blockDim.x + tid;
     if (idx >= (long long)n * n)
         return;
     const int a = (int)(idx / n), c = (int)(idx - (long long)a * n);
+    const int nb0 = csd_nbits(s_max0), nb1 = csd_nbits(s_max1);
     long long d0 = 0, d1 = 0;
     for (int i = 0; i < n_in; ++i) {
         float x = aug[(size_t)i * n + a], y = aug[(size_t)i * n + c];
-        d0 += csd_weight((int32_t)fsub(x, y));
-        d1 += csd_weight((int32_t)fadd(x, y));
+        d0 += csd_count_i32(trunc_i32(fsub(x, y)), nb0);
+        d1 += csd_count_i32(trunc_i32(fadd(x, y)), nb1);
     }
     sign[idx] = (d1 - d0 < 0) ? -1 : 1;
     dist[idx] = (int)min(d0, d1);

@@ -25,18 +25,13 @@ __global__ void int_csd_kernel(const int *x, int n, int nbits, int8_t *csd) {
     int idx = blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= n)
         return;
-    int v = x[idx];
-    for (int k = nbits - 1; k >= 0; --k) {
-        int p2 = (int)(1u << k);
-        int thres = (int)(((long long)p2 * 2) / 3);
-        int d = (v > thres) - (v < -thres);
-        csd[(size_t)idx * nbits + k] = (int8_t)d;
-        v -= p2 * d;
-    }
+    int32_t v = x[idx];
+    for (int k = nbits - 1; k >= 0; --k)
+        csd[(size_t)idx * nbits + k] = (int8_t)csd_digit_i32(v, k);
 }
 __global__ void int_absmax_kernel(const int *x, int n, int *out) {
     int idx = blockIdx.x * blockDim.x + threadIdx.x;
-    int v = idx < n ? abs(x[idx]) : 0;
+    int v = idx < n ? csd_abs(x[idx]) : 0;
     for (int off = 16; off > 0; off >>= 1)
         v = max(v, __shfl_xor_sync(0xffffffffu, v, off));
     if ((threadIdx.x & 31) == 0 && v)
@@ -45,7 +40,7 @@ __global__ void int_absmax_kernel(const int *x, int n, int *out) {
 __global__ void float_to_int_kernel(const float *x, int n, int *out) {
     int idx = blockIdx.x * blockDim.x + threadIdx.x;
     if (idx < n)
-        out[idx] = (int)x[idx];
+        out[idx] = trunc_i32(x[idx]);
 }
 
 } // namespace da
@@ -560,7 +555,7 @@ int da4ml_cmvm_csd_decompose(const float *kernel, int64_t n_in, int64_t n_out, i
             int mx = 0;
             CK(cudaMemcpyAsync(&mx, xi + ne, sizeof(int), cudaMemcpyDeviceToHost, g_stream));
             CK(cudaStreamSynchronize(g_stream));
-            nbits = std::max(1, ceil_log2_pos((double)std::max((float)mx, 1.0f) * 1.5));
+            nbits = csd_nbits(mx);
             int_csd_kernel<<<(unsigned)((ne + 255) / 256), 256, 0, g_stream>>>(xi, (int)ne, nbits, (int8_t *)(b + ocsd));
             memset(shift0, 0, n_in);
             memset(shift1, 0, n_out);
@@ -589,7 +584,7 @@ int da4ml_cmvm_int_arr_to_csd(const int32_t *x, int64_t n, int8_t *csd, int64_t 
         int mx = 0;
         CK(cudaMemcpyAsync(&mx, xi + n, sizeof(int), cudaMemcpyDeviceToHost, g_stream));
         CK(cudaStreamSynchronize(g_stream));
-        int nbits = std::max(1, ceil_log2_pos((double)std::max((float)mx, 1.0f) * 1.5));
+        int nbits = csd_nbits(mx);
         int_csd_kernel<<<(unsigned)((n + 255) / 256), 256, 0, g_stream>>>(xi, (int)n, nbits, (int8_t *)(b + oc));
         CK(cudaGetLastError());
         CK(cudaMemcpyAsync(csd, b + oc, (size_t)n * nbits, cudaMemcpyDeviceToHost, g_stream));

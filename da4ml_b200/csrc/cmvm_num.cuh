@@ -104,6 +104,34 @@ DA_HD int64_t trunc_i64(float v) {
     return (int64_t)v;
 }
 
+// static_cast<int32_t>(float) with x86 cvttss2si semantics: INT32_MIN for NaN, +-inf and |v| >= 2^31 (bit_decompose.cc:59,
+// mat_decompose.cc:81-82).  A plain cast on the device saturates instead, and gives 0 for NaN.
+DA_HD int32_t trunc_i32(float v) {
+    if (!(v > -2147483904.0f && v < 2147483648.0f)) // -2147483904 is the float below -2^31
+        return INT32_MIN;
+    return (int32_t)v;
+}
+
+// One step of the CSD digit loop (bit_decompose.cc:33-39) in the wrapping int32 arithmetic the reference compiles to:
+// at n = 31 the threshold `_2pn * 2 / 3` is 0, at n = 30 it is -(2^31 / 3), and `x -= _2pn * d` wraps.  Returns the
+// digit of weight 2^n and leaves the remainder in x.
+DA_HD int csd_digit_i32(int32_t &x, int n) {
+    const uint32_t p2 = 1u << n;
+    const int32_t thres = (int32_t)(p2 * 2u) / 3;
+    const int d = (x > thres) - (x < -thres);
+    x = (int32_t)((uint32_t)x - p2 * (uint32_t)d);
+    return d;
+}
+
+// |x| as it enters the width max (bit_decompose.cc:23): |INT32_MIN| wraps to itself there and never wins the max.
+DA_HD int32_t csd_abs(int32_t x) { return x == INT32_MIN ? 0 : (x < 0 ? -x : x); }
+
+// CSD width N of values whose largest csd_abs is max_abs (bit_decompose.cc:24-27)
+DA_HD int csd_nbits(int32_t max_abs) {
+    const int n = ceil_log2_pos((double)fmaxf((float)max_abs, 1.0f) * 1.5);
+    return n > 1 ? n : 1;
+}
+
 // indexers.hh:12-18
 DA_HD int8_t iceil_log2(float x) {
     uint32_t bits = f2u(x);
@@ -306,6 +334,18 @@ DA_HD int csd_weight(int32_t x) {
 #else
     return __builtin_popcountll(c);
 #endif
+}
+
+// Non-zero digits of x among the nbits digits of the loop (csd_digit_i32).  Up to 30 digits and 3|x| <= 2^(nbits+1)
+// that is the non-adjacent form's weight; otherwise (the wrapped thresholds of 31 and 32 digits, INT32_MIN, or a value
+// whose float rounded down to a narrower width) the loop runs.
+DA_HD int csd_count_i32(int32_t x, int nbits) {
+    if (nbits <= 30 && x != INT32_MIN && 3 * (int64_t)csd_abs(x) <= (int64_t)2 << nbits)
+        return csd_weight(x);
+    int c = 0;
+    for (int n = nbits - 1; n >= 0; --n)
+        c += csd_digit_i32(x, n) != 0;
+    return c;
 }
 
 } // namespace da

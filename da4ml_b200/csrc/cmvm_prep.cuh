@@ -52,29 +52,24 @@ __global__ void __launch_bounds__(256) cmvm_prep_kernel(ProblemDesc *probs) {
         int i = idx / n_out, j = idx - i * n_out;
         float v = (float)((double)p.kernel[idx] * exp2(-(double)p.shift1[j]));
         v = (float)((double)v * exp2(-(double)p.shift0[i]));
-        int x = (int)v;
-        lmax = max(lmax, abs(x));
+        lmax = max(lmax, csd_abs(trunc_i32(v)));
     }
     atomicMax(&s_max, lmax);
     __syncthreads();
-    int N = ceil_log2_pos((double)fmaxf((float)s_max, 1.0f) * 1.5);
-    N = max(N, 1);
+    const int N = csd_nbits(s_max);
     // digits (bit_decompose.cc:29-38) -> sign planes; zero rows of zero-range inputs (state_opr.cc:92-97)
     for (int idx = tid; idx < n_in * n_out; idx += nt) {
         int i = idx / n_out, j = idx - i * n_out;
         float v = (float)((double)p.kernel[idx] * exp2(-(double)p.shift1[j]));
         v = (float)((double)v * exp2(-(double)p.shift0[i]));
-        int x = (int)v;
+        int32_t x = trunc_i32(v);
         uint32_t P = 0, Nn = 0;
         for (int n = N - 1; n >= 0; --n) {
-            int p2 = (int)(1u << n);
-            int thres = (int)(((long long)p2 * 2) / 3);
-            int d = (x > thres) - (x < -thres);
+            const int d = csd_digit_i32(x, n);
             if (d > 0)
                 P |= 1u << n;
             if (d < 0)
                 Nn |= 1u << n;
-            x -= p2 * d;
         }
         if (p.qint[3 * i] == 0.0f && p.qint[3 * i + 1] == 0.0f) {
             P = 0;
