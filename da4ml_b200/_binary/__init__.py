@@ -42,6 +42,14 @@ _L.da4ml_cmvm_solve.argtypes = [_f32p, C.c_int64, C.c_int64, C.c_char_p, C.c_cha
 _L.da4ml_cmvm_solve_batch.argtypes = [C.c_int64, C.POINTER(_f32p), _i64p, _i64p, C.c_char_p, C.c_char_p, C.c_int, C.c_int, C.POINTER(_f32p), C.POINTER(_f32p), C.c_int, C.c_int, C.c_int, C.POINTER(_vp)]
 _L.da4ml_cmvm_solve_batch_device.argtypes = [C.c_int64, C.POINTER(_vp), _i64p, _i64p, C.c_char_p, C.c_char_p, C.c_int, C.c_int, C.POINTER(_f32p), C.POINTER(_f32p), C.c_int, C.c_int, C.c_int, C.POINTER(_vp)]
 _L.da4ml_cmvm_solve_single.argtypes = [_f32p, C.c_int64, C.c_int64, C.c_char_p, _f32p, _f32p, C.c_int, C.c_int, _i32p, C.c_int64, C.POINTER(_vp)]
+_L.da4ml_cmvm_solve_sweep.argtypes = [_f32p, C.c_int64, C.c_int64, _f32p, _f32p, C.c_int, C.c_int, C.c_int64, C.POINTER(C.c_char_p), C.POINTER(C.c_char_p), _i32p, _i32p, _i32p, C.c_int, C.POINTER(_vp)]
+_L.da4ml_sweep_counts.argtypes = [_vp, _i64p]
+_L.da4ml_sweep_profile.argtypes = [_vp, C.POINTER(C.c_double)]
+_L.da4ml_sweep_summary.argtypes = [_vp, _i64p, _f32p]
+_L.da4ml_sweep_pipeline.argtypes = [_vp, C.c_int64, C.POINTER(_vp)]
+_L.da4ml_sweep_free.argtypes = [_vp]
+_L.da4ml_sweep_free.restype = None
+_L.da4ml_sweep_front.argtypes = [_f32p, _f32p, C.c_int64, _i8p]
 _L.da4ml_pipeline_free.argtypes = [_vp]
 _L.da4ml_pipeline_n_stages.restype = C.c_int64
 _L.da4ml_pipeline_n_stages.argtypes = [_vp]
@@ -79,7 +87,8 @@ EXPORTED_SYMBOLS = [
     'da4ml_cmvm_csd_decompose', 'da4ml_cmvm_int_arr_to_csd', 'da4ml_cmvm_kernel_decompose',
     'da4ml_cmvm_get_lsb_loc', 'da4ml_cmvm_iceil_log2', 'da4ml_cmvm_cost_add', 'da4ml_dais_run',
     'da4ml_dais_program_load', 'da4ml_dais_program_info', 'da4ml_dais_program_run', 'da4ml_dais_program_run_stream',
-    'da4ml_dais_program_free', 'da4ml_dais_program_profile', 'da4ml_dais_program_dump',
+    'da4ml_dais_program_free', 'da4ml_dais_program_profile', 'da4ml_dais_program_dump', 'da4ml_cmvm_solve_sweep', 'da4ml_sweep_counts',
+    'da4ml_sweep_profile', 'da4ml_sweep_summary', 'da4ml_sweep_pipeline', 'da4ml_sweep_free', 'da4ml_sweep_front',
 ]  # fmt: skip
 
 COUNTER_NAMES = ['status', 'n_ops', 'T', 'sum_F', 'sum_R', 'F0', 'R0', 'D_final', 'F_max', 'compactions', 'D0', 'n_bits', 'group_ctas',
@@ -363,6 +372,113 @@ def solve_single_raw(kernel, method='wmc', qintervals=None, latencies=None, adde
     return raw, (tr[: min(trace_cap, raw.counters[0]['T'])] if trace_cap > 0 else None)
 
 
+METHODS = ['mc', 'mc-dc', 'mc-pdc', 'wmc', 'wmc-dc', 'wmc-pdc', 'dummy']  # the library's method codes
+SWEEP_SET_DEFAULTS = dict(method0='wmc', method1='auto', hard_dc=-1, decompose_dc=-2, search_all_decompose_dc=True)  # as solve()
+_SWEEP_INT_FIELDS = ['set', 'hard_dc', 'decompose_dc_start', 'method0', 'method1', 'decompose_dc', 'n_adders', 'n_ops0', 'n_ops1', 'winner', 'front', 'kept']
+_SWEEP_FLOAT_FIELDS = ['cost', 'latency_min', 'latency_max']
+
+
+def sweep_front(cost, latency_max) -> np.ndarray:
+    """Indices of the candidates no other candidate dominates on ``(cost, latency_max)`` (<= on both, < on one); of
+    exactly equal points only the first.  The rule ``solve_sweep`` applies, on the host (no device needed)."""
+    c = np.ascontiguousarray(cost, dtype=np.float32).ravel()
+    l = np.ascontiguousarray(latency_max, dtype=np.float32).ravel()
+    if c.shape != l.shape:
+        raise ValueError(f'cost and latency_max differ in length ({c.size} != {l.size})')
+    f = np.zeros(c.size, np.int8)
+    _check(_L.da4ml_sweep_front(_fp(c), _fp(l), c.size, f.ctypes.data_as(_i8p)))
+    return np.flatnonzero(f)
+
+
+class SweepResult:
+    """One matrix solved under many option sets (``solve_sweep``).
+
+    ``candidates`` holds one numpy array per field, one entry per candidate (set order, then ``decompose_dc`` order):
+    ``set``, ``hard_dc`` and ``decompose_dc_start`` (the H and d its ``_solve`` started with), ``method0`` / ``method1``
+    (after the ``method1='auto'`` and ``hard_dc=0`` rules and any forced ``wmc-dc`` retry), the final ``decompose_dc``,
+    ``cost`` (float32, summed over both stages in op order, the value the argmin uses), ``n_adders``, ``latency_min`` /
+    ``latency_max`` (``Pipeline.latency``), ``n_ops0`` / ``n_ops1``, and the flags ``winner``, ``front``, ``kept`` (op
+    tables available through ``raw`` / ``pipeline``).  ``front`` and ``winners`` are index arrays; ``winners[s]`` is set
+    ``s``'s result, what ``solve(kernel, **option_sets[s])`` returns."""
+
+    def __init__(self, handle, kernel, option_sets, qintervals, latencies, adder_size, carry_size):
+        self._h = handle
+        self.kernel, self.option_sets = kernel, option_sets
+        self._call = dict(qintervals=qintervals, latencies=latencies, adder_size=adder_size, carry_size=carry_size)
+        cnt = np.zeros(4, np.int64)
+        _check(_L.da4ml_sweep_counts(handle, _ip(cnt)))
+        self.n_sets, n, self.n_kept, self.n_solved = (int(v) for v in cnt)
+        ints = np.zeros((n, len(_SWEEP_INT_FIELDS)), np.int64)
+        floats = np.zeros((n, len(_SWEEP_FLOAT_FIELDS)), np.float32)
+        _check(_L.da4ml_sweep_summary(handle, _ip(ints), _fp(floats)))
+        cand = {k: ints[:, i].copy() for i, k in enumerate(_SWEEP_INT_FIELDS)}
+        for k in ('method0', 'method1'):
+            cand[k] = np.asarray(METHODS, dtype=object)[cand[k]].astype(str)
+        for k in ('winner', 'front', 'kept'):
+            cand[k] = cand[k].astype(bool)
+        cand.update({k: floats[:, i].copy() for i, k in enumerate(_SWEEP_FLOAT_FIELDS)})
+        self.candidates = cand
+        self.front = np.flatnonzero(cand['front'])
+        self.winners = np.asarray([int(np.flatnonzero(cand['winner'] & (cand['set'] == s))[0]) for s in range(self.n_sets)], np.int64)
+        prof = (C.c_double * 8)()
+        _check(_L.da4ml_sweep_profile(handle, prof))
+        self.profile = dict(device_ms=prof[0], launches=int(prof[1]), solve_kernel_ms=prof[2], solve_kernel_launches=int(prof[3]), algo_bytes=prof[4],
+                            jobs_total=int(prof[5]), jobs_run=int(prof[6]), candidates=n, candidates_solved=self.n_solved, candidates_kept=self.n_kept)
+
+    def __len__(self):
+        return len(self.candidates['set'])
+
+    def __del__(self):
+        h, self._h = getattr(self, '_h', None), None
+        if h:
+            _L.da4ml_sweep_free(h)
+
+    def raw(self, i: int) -> RawPipeline:
+        """Candidate ``i`` as a ``RawPipeline``; ``ValueError`` when its op tables were not kept."""
+        h = _vp()
+        _check(_L.da4ml_sweep_pipeline(self._h, int(i), C.byref(h)))
+        return RawPipeline(h)
+
+    def pipeline(self, i: int, types_module=None):
+        return self.raw(i).to_pipeline(types_module)
+
+    def reference_call(self, i: int) -> dict:
+        """Keyword arguments of the ``solve(kernel, **kw)`` call whose result candidate ``i`` is."""
+        c = self.candidates
+        s = {**SWEEP_SET_DEFAULTS, **self.option_sets[int(c['set'][i])]}
+        return dict(method0=s['method0'], method1=s['method1'], hard_dc=int(c['hard_dc'][i]), decompose_dc=int(c['decompose_dc_start'][i]),
+                    search_all_decompose_dc=False, **self._call)
+
+
+def solve_sweep(kernel, option_sets, qintervals=None, latencies=None, adder_size=-1, carry_size=-1, keep_all=False) -> SweepResult:
+    """Solve one matrix under every option set of ``option_sets`` in one GPU pass.
+
+    Each option set is a dict of ``solve`` keywords (``method0, method1, hard_dc, decompose_dc,
+    search_all_decompose_dc``; missing keys take ``solve``'s defaults).  The intervals, latencies and the cost model
+    (``adder_size``, ``carry_size``) are shared by all sets: costs under different cost models are not comparable.
+    Op tables come back for the winners and the front, or for every candidate with ``keep_all``."""
+    k = _kernel_arg(kernel)
+    sets = [dict(s) for s in option_sets]
+    for s in sets:
+        bad = set(s) - set(SWEEP_SET_DEFAULTS)
+        if bad:
+            raise TypeError(f'unsupported keys in a sweep option set: {sorted(bad)} (adder_size / carry_size are arguments of the sweep itself)')
+    q = _qint_arg(qintervals, k.shape[0])
+    l = _lat_arg(latencies, k.shape[0])
+    full = [{**SWEEP_SET_DEFAULTS, **s} for s in sets]
+    n = len(full)
+    m0 = (C.c_char_p * max(n, 1))(*[str(s['method0']).encode() for s in full])
+    m1 = (C.c_char_p * max(n, 1))(*[str(s['method1']).encode() for s in full])
+    hdc = np.asarray([int(s['hard_dc']) for s in full] or [0], np.int32)
+    ddc = np.asarray([int(s['decompose_dc']) for s in full] or [0], np.int32)
+    sa = np.asarray([int(bool(s['search_all_decompose_dc'])) for s in full] or [0], np.int32)
+    h = _vp()
+    i32 = lambda a: a.ctypes.data_as(_i32p)  # noqa: E731
+    _check(_L.da4ml_cmvm_solve_sweep(_fp(k), k.shape[0], k.shape[1], _fp(q), _fp(l), int(adder_size), int(carry_size), n, m0, m1, i32(hdc), i32(ddc), i32(sa),
+                                     int(bool(keep_all)), C.byref(h)))
+    return SweepResult(h, k, sets, None if q is None else [tuple(map(float, r)) for r in q], None if l is None else [float(v) for v in l], int(adder_size), int(carry_size))
+
+
 def csd_decompose(inp, center=True):
     """(csd int8[n_in,n_out,N], shift0 int8[n_in], shift1 int8[n_out])  (bindings.cc:63-103)."""
     k = _kernel_arg(inp)
@@ -428,6 +544,6 @@ def cost_add(q0, q1, shift: int, sub: bool, adder_size: int, carry_size: int):
 
 
 __all__ = [
-    'solve', 'solve_batch', 'solve_raw', 'solve_batch_raw', 'solve_batch_device_raw', 'solve_single_raw', 'csd_decompose', 'int_arr_to_csd',
+    'solve', 'solve_batch', 'solve_raw', 'solve_batch_raw', 'solve_batch_device_raw', 'solve_single_raw', 'solve_sweep', 'SweepResult', 'sweep_front', 'csd_decompose', 'int_arr_to_csd',
     'kernel_decompose', 'get_lsb_loc', 'iceil_log2', 'cost_add', 'dais_interp_run', 'device_info', 'plan', 'set_stream', 'set_group_size', 'set_accounting',
 ]  # fmt: skip

@@ -52,6 +52,10 @@ struct da4ml_pipeline {
     std::unique_ptr<PipelineImpl> impl;
 };
 
+struct da4ml_sweep {
+    std::unique_ptr<SweepImpl> impl;
+};
+
 // ---- DAIS interpreter engine ------------------------------------------------------------------------------------------
 // A loaded program: the validated host form plus its device copy (ops, level order, header arrays, table offsets and
 // tables), uploaded on first use on a device and kept until the handle is freed.
@@ -348,7 +352,7 @@ int da4ml_cmvm_solve_batch(
         if (n_problems <= 0 || !kernels || !n_in || !n_out || !out || !method0 || !method1)
             throw ApiError(DA4ML_E_INVALID, "invalid argument");
         std::vector<std::unique_ptr<PipelineImpl>> res;
-        solve_many(n_problems, kernels, n_in, n_out, method0, method1, hard_dc, decompose_dc, qintervals, latencies, adder_size, carry_size, search_all != 0, res);
+        solve_many(n_problems, kernels, n_in, n_out, {SolveOptions{method0, method1, hard_dc, decompose_dc, search_all != 0}}, qintervals, latencies, adder_size, carry_size, res);
         for (int64_t i = 0; i < n_problems; ++i) {
             out[i] = new da4ml_pipeline();
             out[i]->impl = std::move(res[i]);
@@ -365,7 +369,7 @@ int da4ml_cmvm_solve_batch_device(
         if (n_problems <= 0 || !kernels_dev || !n_in || !n_out || !out || !method0 || !method1)
             throw ApiError(DA4ML_E_INVALID, "invalid argument");
         std::vector<std::unique_ptr<PipelineImpl>> res;
-        solve_many(n_problems, kernels_dev, n_in, n_out, method0, method1, hard_dc, decompose_dc, qintervals, latencies, adder_size, carry_size, search_all != 0, res, true);
+        solve_many(n_problems, kernels_dev, n_in, n_out, {SolveOptions{method0, method1, hard_dc, decompose_dc, search_all != 0}}, qintervals, latencies, adder_size, carry_size, res, true);
         for (int64_t i = 0; i < n_problems; ++i) {
             out[i] = new da4ml_pipeline();
             out[i]->impl = std::move(res[i]);
@@ -429,6 +433,98 @@ int da4ml_cmvm_solve_single(
         *out = new da4ml_pipeline();
         (*out)->impl = std::move(pl);
     });
+}
+
+// ---- sweep: one matrix under many option sets ----------------------------------------------------
+int da4ml_cmvm_solve_sweep(
+    const float *kernel, int64_t n_in, int64_t n_out, const float *qintervals, const float *latencies, int adder_size, int carry_size, int64_t n_sets,
+    const char *const *method0, const char *const *method1, const int32_t *hard_dc, const int32_t *decompose_dc, const int32_t *search_all, int keep_all,
+    da4ml_sweep_t **out
+) {
+    return guarded([&] {
+        if (!kernel || n_in <= 0 || n_out <= 0)
+            throw ApiError(DA4ML_E_INVALID, "solve_sweep: kernel must be a non-empty 2D array");
+        if (n_sets <= 0)
+            throw ApiError(DA4ML_E_INVALID, "solve_sweep: n_sets must be positive (got " + std::to_string(n_sets) + ")");
+        if (!method0 || !method1 || !hard_dc || !decompose_dc || !search_all)
+            throw ApiError(DA4ML_E_INVALID, "solve_sweep: an option array is null");
+        if (!out)
+            throw ApiError(DA4ML_E_INVALID, "solve_sweep: out is null");
+        std::vector<SolveOptions> sets((size_t)n_sets);
+        for (int64_t s = 0; s < n_sets; ++s) {
+            if (!method0[s] || !method1[s])
+                throw ApiError(DA4ML_E_INVALID, "solve_sweep: a method of option set " + std::to_string(s) + " is null");
+            sets[s] = SolveOptions{method0[s], method1[s], hard_dc[s], decompose_dc[s], search_all[s] != 0};
+            parse_method(sets[s].method0); // "Unknown method: ..." before any device call
+            if (sets[s].method1 != "auto")
+                parse_method(sets[s].method1);
+        }
+        auto sw = std::make_unique<SweepImpl>();
+        std::vector<std::unique_ptr<PipelineImpl>> winners;
+        solve_many(1, &kernel, &n_in, &n_out, sets, &qintervals, &latencies, adder_size, carry_size, winners, false, sw.get(), keep_all != 0);
+        *out = new da4ml_sweep{std::move(sw)};
+    });
+}
+
+int da4ml_sweep_counts(const da4ml_sweep_t *s, int64_t out[4]) {
+    if (!s || !out)
+        return DA4ML_E_INVALID;
+    out[0] = s->impl->n_sets;
+    out[1] = (int64_t)s->impl->cands.size();
+    out[2] = (int64_t)std::count_if(s->impl->kept.begin(), s->impl->kept.end(), [](const std::unique_ptr<PipelineImpl> &p) { return p != nullptr; });
+    out[3] = s->impl->n_solved;
+    return DA4ML_OK;
+}
+
+int da4ml_sweep_profile(const da4ml_sweep_t *s, double out[8]) {
+    if (!s || !out)
+        return DA4ML_E_INVALID;
+    const PipelineImpl &t = s->impl->totals;
+    const double row[8] = {t.device_ms, (double)t.launches, t.solve_ms, (double)t.solve_launches, t.algo_bytes, (double)t.jobs_total, (double)t.jobs_run, 0.0};
+    std::copy(row, row + 8, out);
+    return DA4ML_OK;
+}
+
+int da4ml_sweep_summary(const da4ml_sweep_t *s, int64_t *ints, float *floats) {
+    if (!s)
+        return DA4ML_E_INVALID;
+    for (size_t i = 0; i < s->impl->cands.size(); ++i) {
+        const CandidateSummary &c = s->impl->cands[i];
+        if (ints) {
+            const int64_t row[12] = {c.set, c.hard_dc, c.decompose_dc_start, c.method0, c.method1, c.decompose_dc, c.n_adders, c.n_ops0, c.n_ops1, c.winner, c.front,
+                                     s->impl->kept[i] != nullptr};
+            std::copy(row, row + 12, ints + 12 * i);
+        }
+        if (floats) {
+            floats[3 * i + 0] = c.cost;
+            floats[3 * i + 1] = c.latency_min;
+            floats[3 * i + 2] = c.latency_max;
+        }
+    }
+    return DA4ML_OK;
+}
+
+int da4ml_sweep_pipeline(const da4ml_sweep_t *s, int64_t candidate, da4ml_pipeline_t **out) {
+    return guarded([&] {
+        if (!s || !out)
+            throw ApiError(DA4ML_E_INVALID, "sweep_pipeline: invalid argument");
+        const int64_t n = (int64_t)s->impl->cands.size();
+        if (candidate < 0 || candidate >= n)
+            throw ApiError(DA4ML_E_INVALID, "sweep_pipeline: candidate " + std::to_string(candidate) + " is out of range [0, " + std::to_string(n) + ")");
+        if (!s->impl->kept[candidate])
+            throw ApiError(DA4ML_E_INVALID, "sweep_pipeline: the op tables of candidate " + std::to_string(candidate) +
+                                                " were not kept (only the winners and the front are, unless the sweep was run with keep_all)");
+        *out = new da4ml_pipeline{std::make_unique<PipelineImpl>(*s->impl->kept[candidate])};
+    });
+}
+
+void da4ml_sweep_free(da4ml_sweep_t *s) { delete s; }
+
+int da4ml_sweep_front(const float *cost, const float *latency_max, int64_t n, int8_t *front) {
+    if (n < 0 || (n > 0 && (!cost || !latency_max || !front)))
+        return DA4ML_E_INVALID;
+    pareto_front(cost, latency_max, n, front);
+    return DA4ML_OK;
 }
 
 void da4ml_pipeline_free(da4ml_pipeline_t *p) { delete p; }

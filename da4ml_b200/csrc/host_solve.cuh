@@ -2,6 +2,8 @@
 // solve_single of every candidate of every problem goes into one launch per round.
 #pragma once
 #include "host_stage.cuh"
+#include <map>
+#include <tuple>
 
 namespace da {
 
@@ -17,6 +19,49 @@ struct PipelineImpl {
     int64_t launches = 0, solve_launches = 0;
     int64_t jobs_total = 0, jobs_run = 0; // solve_single jobs the reference would execute / executed after sharing identical ones
 };
+
+// One option set of `solve` (api.cc:147-158): every argument but the matrix, its input intervals / latencies and the cost
+// model (adder_size, carry_size), which a call shares across its option sets.
+struct SolveOptions {
+    std::string method0 = "wmc", method1 = "auto";
+    int hard_dc = -1, decompose_dc = -2;
+    bool search_all = true;
+};
+
+// A sweep's report on one candidate, i.e. one decompose_dc try of one option set (api.cc:190-201): the design that
+// solve(W, method0, method1, hard_dc, decompose_dc_start, search_all_decompose_dc=false, ...) returns.
+struct CandidateSummary {
+    int set = 0;
+    int hard_dc = -1, decompose_dc_start = -2; // what its _solve was started with (hard_dc = 1e9 for an unbounded search)
+    int method0 = 0, method1 = 0;              // Method after api.cc:41-51 and any forced wmc-dc retry (api.cc:84-93)
+    int decompose_dc = 0;                      // after the api.cc:74-80 clamp and the latency retries
+    float cost = 0.0f;                         // float sum over both stages in op order (api.cc:222-227)
+    float latency_min = 0.0f, latency_max = 0.0f;
+    int64_t n_adders = 0, n_ops0 = 0, n_ops1 = 0;
+    bool winner = false, front = false;
+};
+
+struct SweepImpl {
+    int64_t n_sets = 0, n_solved = 0;  // option sets; distinct candidates actually solved
+    std::vector<CandidateSummary> cands; // set order, then decompose_dc order
+    std::vector<std::unique_ptr<PipelineImpl>> kept; // per candidate: both stages with op tables, or null
+    PipelineImpl totals; // counters of the whole call (no stages)
+};
+
+// The candidates no other candidate dominates on (cost, latency_max): j dominates i when it is <= on both and < on one.
+// Of candidates with exactly equal (cost, latency_max) only the first is on the front.
+static void pareto_front(const float *cost, const float *latency_max, int64_t n, int8_t *front) {
+    for (int64_t i = 0; i < n; ++i) {
+        bool on = true;
+        for (int64_t j = 0; j < n && on; ++j) {
+            if (j == i || !(cost[j] <= cost[i] && latency_max[j] <= latency_max[i]))
+                continue;
+            const bool better = cost[j] < cost[i] || latency_max[j] < latency_max[i];
+            on = !(better || j < i);
+        }
+        front[i] = on;
+    }
+}
 
 struct Candidate {
     // fixed
@@ -104,19 +149,27 @@ static float stage_max_latency(const StageResult &r) {
     return m;
 }
 
+// Every problem is solved under every option set of `sets`.  out[problem * sets.size() + set] receives the winner, the
+// result of solve(W, **set).  With `sweep` (one problem only) every candidate is summarised there instead, and the op
+// tables of the winners and of the front (of every candidate with keep_all) are kept; `out` stays empty.
 static void solve_many(
-    int64_t n_problems, const float *const *kernels, const int64_t *n_in, const int64_t *n_out, const std::string &method0_in,
-    const std::string &method1_in, int hard_dc, int decompose_dc, const float *const *qints, const float *const *lats,
-    int adder_size, int carry_size, bool search_all, std::vector<std::unique_ptr<PipelineImpl>> &out, bool kernels_on_device = false
+    int64_t n_problems, const float *const *kernels, const int64_t *n_in, const int64_t *n_out, const std::vector<SolveOptions> &sets,
+    const float *const *qints, const float *const *lats, int adder_size, int carry_size, std::vector<std::unique_ptr<PipelineImpl>> &out,
+    bool kernels_on_device = false, SweepImpl *sweep = nullptr, bool keep_all = false
 ) {
     init_device();
     g_out_arena2.reset();
     Timing tm;
     int64_t jobs_total = 0, jobs_run = 0;
+    const int n_sets = (int)sets.size();
+    if (n_sets <= 0 || (sweep && n_problems != 1))
+        throw ApiError(DA4ML_E_INVALID, "invalid argument");
     // validate methods up front (the reference throws from the worker, api.cc:231-240)
-    parse_method(method0_in);
-    if (method1_in != "auto")
-        parse_method(method1_in);
+    for (const SolveOptions &o : sets) {
+        parse_method(o.method0);
+        if (o.method1 != "auto")
+            parse_method(o.method1);
+    }
 
     std::vector<Problem> probs(n_problems);
     std::vector<Candidate> cands;
@@ -178,18 +231,14 @@ static void solve_many(
             o += bytes;
         }
     }
-    // ---- candidates (api.cc:176-201)
+    // ---- candidates (api.cc:176-201).  Each (problem, set, try) is an entry; tries that start _solve in the same state
+    // (methods after api.cc:41-51, hard_dc, decompose_dc after the api.cc:74-80 clamp) are one candidate, solved once.
+    struct Entry {
+        int problem, set, hard_dc, dc_start, cand;
+    };
+    std::vector<Entry> entries;
     for (int64_t pi = 0; pi < n_problems; ++pi) {
         Problem &P = probs[pi];
-        std::vector<std::pair<int, int>> tries; // (hard_dc passed to _solve, decompose_dc passed to _solve)
-        if (!search_all)
-            tries.push_back({hard_dc, decompose_dc});
-        else {
-            int _hard_dc = hard_dc < 0 ? 1000000000 : hard_dc;
-            int max_dc = std::min(_hard_dc, (int)std::ceil(std::log2((float)P.n_in)));
-            for (int d = -1; d <= max_dc; ++d)
-                tries.push_back({_hard_dc, d});
-        }
         // latency_allowed = hard_dc + minimal latency (api.cc:72) is only ever COMPARED with stage latencies (api.cc:117,133).
         // With search_all the reference passes hard_dc = 1e9 when the caller gave none: as long as every latency of the graph
         // stays far below that (input latencies < 1e6; an adder adds at most 64 and there are < 1e6 of them), no comparison
@@ -197,26 +246,47 @@ static void solve_many(
         bool latencies_small = true;
         for (float v : P.lat)
             latencies_small = latencies_small && std::isfinite(v) && std::fabs(v) < 1e6f;
-        for (auto &tr : tries) {
-            Candidate c;
-            c.problem = (int)pi;
-            c.method0 = method0_in;
-            c.method1 = method1_in;
-            c.hard_dc = tr.first;
-            c.adder_size = adder_size;
-            c.carry_size = carry_size;
-            // api.cc:41-51
-            if (c.method1 == "auto")
-                c.method1 = (c.hard_dc >= 6 || ends_with(c.method0, "dc")) ? c.method0 : c.method0 + "-dc";
-            if (c.hard_dc == 0 && !ends_with(c.method0, "dc"))
-                c.method0 = c.method0 + "-dc";
-            // api.cc:74-80
-            int log2_n = (int)std::ceil(std::log2((float)P.n_in));
-            c.decompose_dc = tr.second == -2 ? std::min(c.hard_dc, log2_n) : std::min({c.hard_dc, tr.second, log2_n});
-            if (c.hard_dc >= 0 && !(c.hard_dc >= 100000000 && latencies_small))
-                P.need_min_lat = true; // (see below: a delay bound of 1e9 can never bind)
-            P.cand.push_back((int)cands.size());
-            cands.push_back(std::move(c));
+        std::map<std::tuple<std::string, std::string, int, int>, int> seen;
+        for (int si = 0; si < n_sets; ++si) {
+            const SolveOptions &o = sets[si];
+            std::vector<std::pair<int, int>> tries; // (hard_dc passed to _solve, decompose_dc passed to _solve)
+            if (!o.search_all)
+                tries.push_back({o.hard_dc, o.decompose_dc});
+            else {
+                int _hard_dc = o.hard_dc < 0 ? 1000000000 : o.hard_dc;
+                int max_dc = std::min(_hard_dc, (int)std::ceil(std::log2((float)P.n_in)));
+                for (int d = -1; d <= max_dc; ++d)
+                    tries.push_back({_hard_dc, d});
+            }
+            for (auto &tr : tries) {
+                Candidate c;
+                c.problem = (int)pi;
+                c.method0 = o.method0;
+                c.method1 = o.method1;
+                c.hard_dc = tr.first;
+                c.adder_size = adder_size;
+                c.carry_size = carry_size;
+                // api.cc:41-51
+                if (c.method1 == "auto")
+                    c.method1 = (c.hard_dc >= 6 || ends_with(c.method0, "dc")) ? c.method0 : c.method0 + "-dc";
+                if (c.hard_dc == 0 && !ends_with(c.method0, "dc"))
+                    c.method0 = c.method0 + "-dc";
+                // api.cc:74-80
+                int log2_n = (int)std::ceil(std::log2((float)P.n_in));
+                c.decompose_dc = tr.second == -2 ? std::min(c.hard_dc, log2_n) : std::min({c.hard_dc, tr.second, log2_n});
+                const auto key = std::make_tuple(c.method0, c.method1, c.hard_dc, c.decompose_dc);
+                const auto it = seen.find(key);
+                if (it != seen.end()) {
+                    entries.push_back(Entry{(int)pi, si, tr.first, tr.second, it->second});
+                    continue;
+                }
+                if (c.hard_dc >= 0 && !(c.hard_dc >= 100000000 && latencies_small))
+                    P.need_min_lat = true; // (see below: a delay bound of 1e9 can never bind)
+                seen.emplace(key, (int)cands.size());
+                entries.push_back(Entry{(int)pi, si, tr.first, tr.second, (int)cands.size()});
+                P.cand.push_back((int)cands.size());
+                cands.push_back(std::move(c));
+            }
         }
     }
     // ---- decomposition scratch: one (m0, m1, mapping) triple per candidate
@@ -451,34 +521,86 @@ static void solve_many(
             }
         }
     }
-    // ---- argmin over candidates, first minimum wins (api.cc:243-249); cost summed in float in op order (api.cc:222-227)
-    out.clear();
-    for (auto &P : probs) {
-        int best = -1;
-        float best_cost = 0;
-        for (int ci : P.cand) {
-            Candidate &c = cands[ci];
-            const float cost = c.job1.res.cost_sum; // stage-0 sum carried into stage 1 on the device
-            if (best < 0 || cost < best_cost) {
-                best = ci;
-                best_cost = cost;
+    // ---- argmin over each set's candidates, first minimum wins (api.cc:243-249); cost summed in float in op order
+    // (api.cc:222-227): the stage-0 sum is carried into stage 1 on the device
+    std::vector<int> win((size_t)n_problems * n_sets, -1); // entry index
+    for (size_t e = 0; e < entries.size(); ++e) {
+        int &w = win[(size_t)entries[e].problem * n_sets + entries[e].set];
+        if (w < 0 || cands[entries[e].cand].job1.res.cost_sum < cands[entries[w].cand].job1.res.cost_sum)
+            w = (int)e;
+    }
+    // Only the op tables of what is returned leave the device.  A lone set's winner is used once and can be moved.
+    const bool move_out = n_sets == 1 && !sweep;
+    auto pipeline_of = [&](Candidate &c, bool move) {
+        fetch_ops(c.job0.res);
+        fetch_ops(c.job1.res);
+        auto pl = std::make_unique<PipelineImpl>();
+        pl->stages.push_back(move ? std::move(c.job0.res) : c.job0.res);
+        pl->stages.push_back(move ? std::move(c.job1.res) : c.job1.res);
+        return pl;
+    };
+    auto put_totals = [&](PipelineImpl &pl) {
+        pl.device_ms = tm.device_ms;
+        pl.launches = tm.launches;
+        pl.solve_ms = tm.solve_ms;
+        pl.solve_launches = tm.solve_launches;
+        pl.algo_bytes = tm.algo_bytes;
+        pl.jobs_total = jobs_total;
+        pl.jobs_run = jobs_run;
+    };
+    if (sweep) { // (summaries first: the winners below may be moved out of the candidates otherwise)
+        // Pipeline.latency reads ops[out_idx] of the last stage with Python indexing: a dead output (-1) reads the last op
+        std::vector<float4> last_op(cands.size());
+        for (size_t ci = 0; ci < cands.size(); ++ci) {
+            const StageResult &r = cands[ci].job1.res;
+            if (r.n_ops_dev > 0 && std::any_of(r.out_idxs.begin(), r.out_idxs.end(), [](int64_t v) { return v < 0; }))
+                CK(cudaMemcpyAsync(&last_op[ci], r.d_q + (r.n_ops_dev - 1), sizeof(float4), cudaMemcpyDeviceToHost, g_stream));
+        }
+        CK(cudaStreamSynchronize(g_stream));
+        sweep->n_sets = n_sets;
+        sweep->n_solved = (int64_t)cands.size();
+        sweep->cands.assign(entries.size(), CandidateSummary());
+        std::vector<float> cost(entries.size()), lat_max(entries.size());
+        for (size_t e = 0; e < entries.size(); ++e) {
+            const Candidate &c = cands[entries[e].cand];
+            const StageResult &r0 = c.job0.res, &r1 = c.job1.res;
+            CandidateSummary &s = sweep->cands[e];
+            s.set = entries[e].set;
+            s.hard_dc = entries[e].hard_dc;
+            s.decompose_dc_start = entries[e].dc_start;
+            s.method0 = parse_method(c.method0);
+            s.method1 = parse_method(c.method1);
+            s.decompose_dc = c.decompose_dc;
+            s.cost = r1.cost_sum;
+            s.n_ops0 = r0.n_ops_dev;
+            s.n_ops1 = r1.n_ops_dev;
+            s.n_adders = (r0.n_ops_dev - r0.n_in) + (r1.n_ops_dev - r1.n_in); // (each stage's first n_in ops copy its inputs)
+            for (size_t k = 0; k < r1.out_idxs.size(); ++k) {
+                const float l = r1.out_idxs[k] >= 0 ? r1.out_q[k].w : last_op[entries[e].cand].w;
+                s.latency_min = k == 0 ? l : std::min(s.latency_min, l);
+                s.latency_max = k == 0 ? l : std::max(s.latency_max, l);
+            }
+            s.winner = win[(size_t)s.set] == (int)e;
+            cost[e] = s.cost;
+            lat_max[e] = s.latency_max;
+        }
+        std::vector<int8_t> front(entries.size());
+        pareto_front(cost.data(), lat_max.data(), (int64_t)entries.size(), front.data());
+        sweep->kept.resize(entries.size());
+        for (size_t e = 0; e < entries.size(); ++e) {
+            CandidateSummary &s = sweep->cands[e];
+            s.front = front[e] != 0;
+            if (keep_all || s.winner || s.front) {
+                sweep->kept[e] = pipeline_of(cands[entries[e].cand], false);
+                put_totals(*sweep->kept[e]);
             }
         }
-        fetch_ops(cands[best].job0.res); // only the winner's op tables leave the device
-        fetch_ops(cands[best].job1.res);
-        auto pl = std::make_unique<PipelineImpl>();
-        pl->stages.push_back(std::move(cands[best].job0.res));
-        pl->stages.push_back(std::move(cands[best].job1.res));
-        out.push_back(std::move(pl));
+        put_totals(sweep->totals);
     }
-    for (auto &pl : out) {
-        pl->device_ms = tm.device_ms;
-        pl->launches = tm.launches;
-        pl->solve_ms = tm.solve_ms;
-        pl->solve_launches = tm.solve_launches;
-        pl->algo_bytes = tm.algo_bytes;
-        pl->jobs_total = jobs_total;
-        pl->jobs_run = jobs_run;
+    out.clear();
+    for (size_t k = 0; !sweep && k < win.size(); ++k) { // (a sweep hands its winners out through `kept`)
+        out.push_back(pipeline_of(cands[entries[win[k]].cand], move_out));
+        put_totals(*out.back());
     }
 }
 

@@ -52,6 +52,12 @@ struct OutArena {
         cur = 0;
         off = 0;
     }
+    size_t spare() const { // bytes the chunks already allocated can still hand out
+        size_t s = 0;
+        for (size_t k = cur; k < chunks.size(); ++k)
+            s += chunks[k].cap - (k == cur ? off : 0);
+        return s;
+    }
     char *take(size_t bytes) {
         bytes = (bytes + 255) & ~size_t(255);
         while (true) {
@@ -203,6 +209,25 @@ static void run_stage_jobs(std::vector<StageJob *> &jobs, Timing &tm, bool want_
         };
         std::vector<OOff> oo(n);
         long long max_cols = 0, max_colcap = 0, max_heap = 0, max_ecap = 0;
+        // The op tables of every job stay in g_out_arena2 until the call ends (a solve with many candidates, and retries,
+        // keep adding to it): check that the device can hold this round's before carving them.
+        {
+            size_t need = 0;
+            for (int i = 0; i < n; ++i) {
+                const size_t ops_cap = (size_t)todo[i]->n_in + (size_t)pmeta[(size_t)i * PM_WORDS + PM_D0] + 1;
+                for (size_t b : {sizeof(int4) * ops_cap, sizeof(float4) * ops_cap, sizeof(float) * ops_cap, sizeof(float4) * (size_t)todo[i]->n_out})
+                    need += (b + 255) & ~size_t(255);
+            }
+            const size_t spare = g_out_arena2.spare();
+            if (need > spare) {
+                size_t free_b = 0, total_b = 0;
+                CK(cudaMemGetInfo(&free_b, &total_b));
+                if (need - spare + (size_t(256) << 20) > free_b) // (the arena grows in chunks of at least 256 MB)
+                    throw ApiError(DA4ML_E_CAPACITY, "the op tables of " + std::to_string(n) + " solve_single jobs need " + std::to_string(need >> 20) +
+                                                         " MB of device memory and only " + std::to_string(free_b >> 20) +
+                                                         " MB are free; they stay on the device until the call ends, so solve fewer option sets or matrices per call");
+            }
+        }
         for (int i = 0; i < n; ++i) {
             StageJob &j = *todo[i];
             const int *pm = &pmeta[(size_t)i * PM_WORDS];

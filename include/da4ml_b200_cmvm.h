@@ -103,6 +103,45 @@ int da4ml_cmvm_solve_single(
     da4ml_pipeline_t **out
 );
 
+/* ---- sweep: one matrix under many option sets (the reference has no counterpart; its caller calls solve once per set) --
+ * Option set s is {method0[s], method1[s], hard_dc[s], decompose_dc[s], search_all[s]}; the matrix, qintervals /
+ * latencies (NULL -> defaults, as for da4ml_cmvm_solve) and the cost model (adder_size, carry_size) are shared.  Each set
+ * expands into candidates as solve expands it (api.cc:176-201): with search_all, one per d in -1 .. min(H, ceil(log2
+ * n_in)) with H = hard_dc (1e9 when hard_dc < 0), otherwise one with H = hard_dc, d = decompose_dc.  Candidate c is the
+ * result of solve(kernel, method0, method1, H, d, search_all_decompose_dc = 0, ...) bit for bit; each set's winner (its
+ * first candidate of minimum cost, api.cc:243-249) is the result of solve with the set itself.  Candidates are listed in
+ * set order, then d order.  Candidates of different sets that start from the same state are solved once.  All jobs run
+ * together, one launch per round.
+ * The front: the candidates no other candidate dominates on (cost, latency_max), the first of exactly equal points only.
+ * Op tables are kept for the winners and the front, or for every candidate with keep_all.  Arguments are checked on the
+ * host before any device call (DA4ML_E_INVALID; an unknown method gives DA4ML_E_RUNTIME "Unknown method: ...").  If any
+ * set fails as solve would fail, the call fails with that error and returns no result.  DA4ML_E_CAPACITY when the device
+ * cannot hold the op tables of all jobs.  Free with da4ml_sweep_free. */
+typedef struct da4ml_sweep da4ml_sweep_t; /* opaque sweep result */
+int da4ml_cmvm_solve_sweep(
+    const float *kernel, int64_t n_in, int64_t n_out, const float *qintervals, const float *latencies, int adder_size,
+    int carry_size, int64_t n_sets, const char *const *method0, const char *const *method1, const int32_t *hard_dc,
+    const int32_t *decompose_dc, const int32_t *search_all, int keep_all, da4ml_sweep_t **out
+);
+/* counts: {n_sets, n_candidates, n_kept (candidates with op tables), n_solved (distinct candidates solved)} */
+int da4ml_sweep_counts(const da4ml_sweep_t *s, int64_t out[4]);
+/* Profile of the sweep call, as da4ml_pipeline_profile: {device_ms, launches, solve_kernel_ms, solve_kernel_launches,
+ * algorithmic_bytes, jobs_total, jobs_run, 0}. */
+int da4ml_sweep_profile(const da4ml_sweep_t *s, double out[8]);
+/* Per candidate (either pointer may be NULL):
+ *   ints   [n_candidates][12] int64 = {set, H, d (as started), method0, method1 (after api.cc:41-51 and any forced wmc-dc
+ *          retry; 0 mc, 1 mc-dc, 2 mc-pdc, 3 wmc, 4 wmc-dc, 5 wmc-pdc, 6 dummy), final decompose_dc, adders, stage-0 ops,
+ *          stage-1 ops, winner, front, kept}
+ *   floats [n_candidates][3] float32 = {cost (float sum over both stages in op order, api.cc:222-227), latency_min,
+ *          latency_max (Pipeline.latency: the last stage's output latencies)} */
+int da4ml_sweep_summary(const da4ml_sweep_t *s, int64_t *ints, float *floats);
+/* A kept candidate as an ordinary two-stage result (a copy; free with da4ml_pipeline_free).  DA4ML_E_INVALID for a
+ * candidate that was not kept or is out of range. */
+int da4ml_sweep_pipeline(const da4ml_sweep_t *s, int64_t candidate, da4ml_pipeline_t **out);
+void da4ml_sweep_free(da4ml_sweep_t *s);
+/* The front rule on its own (no device): front[i] = 1 when no j dominates i on (cost, latency_max), 0 otherwise. */
+int da4ml_sweep_front(const float *cost, const float *latency_max, int64_t n, int8_t *front);
+
 /* ---- result access (mirrors make_py_comblogic, bindings.cc:106-139) ---------------------------- */
 void da4ml_pipeline_free(da4ml_pipeline_t *p);
 int64_t da4ml_pipeline_n_stages(const da4ml_pipeline_t *p);
