@@ -17,7 +17,7 @@ struct OwnPlan {
 };
 __host__ __device__ inline OwnPlan own_plan(int nchunk_cap, int n_out_max, int e_cap_max, int lcap, int hlog, int narrow) {
     OwnPlan P;
-    size_t o = ((size_t)nchunk_cap * 17 + 15) & ~size_t(15); // chunk caches: 3 x u32 + dirty list (int) + dirty flag (u8)
+    size_t o = (page_cache_bytes(nchunk_cap) + 15) & ~size_t(15); // the page caches (carved in solve_own_kernel_body)
     auto take = [&](size_t bytes) {
         const size_t at = o;
         o += (bytes + 15) & ~size_t(15);
@@ -56,19 +56,18 @@ __device__ void solve_problem_own(const ProblemDesc &p, const Ctx &cx, const Own
     if (tid == 0) {
         b.seg_len = 0;
         {
-            // hot regions for the first expressions this CTA owns: its inputs and the earliest new expressions, the dense
-            // rows that are rewritten again and again (not worth it when a region would be only a few chunks long)
-            const int n_own = (p.e_cap - cx.rank + G - 1) / G, H = min(n_own, DA_HOT_MAX), ch = 1 << cx.cfg.chunk_log;
-            b.cap0 = cx.ws.fseg_cap;
-            b.hot_n = 0;
-            b.hot_cap = 0;
-            if (H > 0) {
-                const int half = (cx.ws.fseg_cap / 4) & ~(ch - 1), hc = ((cx.ws.fseg_cap - half) / H) & ~(ch - 1); // a quarter for the common log
-                if (hc >= 4 * ch)
-                    b.cap0 = half, b.hot_n = H, b.hot_cap = hc;
-            }
+            // hot logs for the first expressions this CTA owns: its inputs and the earliest new expressions, the dense
+            // rows that are rewritten again and again (not when the pool is too small to give each a few pages)
+            const int n_own = (p.e_cap - cx.rank + G - 1) / G, H = min(n_own, DA_HOT_MAX);
+            b.pages = min(cx.ws.fseg_cap >> cx.cfg.chunk_log, cx.cfg.nchunk_cap - 2);
+            b.hot_top = b.pages;
+            b.cap0 = b.pages << cx.cfg.chunk_log;
+            b.n_used = 0;
+            b.n_free = 0;
+            b.hot_n = H > 0 && b.pages >= 8 * H ? H : 0;
+            b.hot_room = 6 * (2 * nbits - 1); // 3 rewritten rows x shifts x signs
             for (int k = 0; k < DA_HOT_MAX; ++k)
-                b.hot_len[k] = b.hot_snap[k] = 0;
+                b.hot_len[k] = b.hot_snap[k] = b.hot_np[k] = 0;
         }
         b.n_new = 0;
         b.live_old = 0;
@@ -132,6 +131,9 @@ __device__ void solve_problem_own(const ProblemDesc &p, const Ctx &cx, const Own
         b.seg_len = min(b.seg_len, b.cap0);
         b.n_new = 0;
     }
+    __syncthreads();
+    if (wid == 0)
+        hot_grow(cx); // the hot logs' first pages
     __syncthreads();
     // Two teams of warps work side by side in a greedy step: the first warps substitute, update and recount (team C,
     // barrier 1), the last quarter brings the argmax caches up to date for the rewritten expressions (team R, barrier 2)
@@ -221,23 +223,12 @@ __device__ void solve_problem_own(const ProblemDesc &p, const Ctx &cx, const Own
         }
         const int seg0 = seg_cur; // what the argmax caches have to cover; this step's entries are appended behind it
         {
-            // a hot input of this CTA is rewritten: every entry of its region dies with it (uniform over the CTA)
+            // a hot expression of this CTA is rewritten: every entry of its log dies with it (uniform over the CTA)
             const bool k0 = (int)(c0 % (uint32_t)G) == cx.rank && (int)(c0 / (uint32_t)G) < b.hot_n;
             const bool k1 = c1 != c0 && (int)(c1 % (uint32_t)G) == cx.rank && (int)(c1 / (uint32_t)G) < b.hot_n;
             if (k0 || k1) {
-                for (int w = 0; w < 2; ++w) {
-                    if (!(w == 0 ? k0 : k1))
-                        continue;
-                    const int k = (int)((w == 0 ? c0 : c1) / (uint32_t)G), cpr = b.hot_cap >> cx.cfg.chunk_log, cb = (b.cap0 >> cx.cfg.chunk_log) + k * cpr;
-                    for (int c = tid; c < cpr; c += nt) {
-                        cx.cb_score[cb + c] = 0u;
-                        cx.cb_khi[cb + c] = 0u;
-                        cx.cb_klo[cb + c] = 0u;
-                        cx.cb_dirty[cb + c] = 0;
-                    }
-                    if (tid == 0)
-                        b.hot_len[k] = b.hot_snap[k] = 0;
-                }
+                const int ks[2] = {(int)(c0 / (uint32_t)G), (int)(c1 / (uint32_t)G)};
+                hot_free(cx, ks, (k0 ? 1u : 0u) | (k1 ? 2u : 0u));
                 __syncthreads();
             }
         }
@@ -256,10 +247,10 @@ __device__ void solve_problem_own(const ProblemDesc &p, const Ctx &cx, const Own
             own_recount(p, cx, ox, tm_c, newid, stamp, thresh, best);
             // maxima of the entries each log received in this step (their chunks' caches are updated behind the join)
             for (int r = wid; r <= b.hot_n; r += nt_c >> 5) {
-                const int base = r == 0 ? 0 : b.cap0 + (r - 1) * b.hot_cap, l0 = r == 0 ? seg0 : b.hot_snap[r - 1];
-                const int l1 = r == 0 ? min(b.seg_len, b.cap0) : min(b.hot_len[r - 1], b.hot_cap);
+                const int l0 = r == 0 ? seg0 : b.hot_snap[r - 1];
+                const int l1 = r == 0 ? min(b.seg_len, b.cap0) : min(b.hot_len[r - 1], b.hot_np[r - 1] << cx.cfg.chunk_log);
                 if (l1 > l0) // (uniform over the warp; most logs receive nothing in a step)
-                    merge_appended_scan(cx, r, base, l0, l1, thresh);
+                    merge_appended_scan(cx, r, l0, l1, thresh);
             }
             DA_LAP(1)
         }
@@ -287,20 +278,25 @@ __device__ void solve_problem_own(const ProblemDesc &p, const Ctx &cx, const Own
         DA_LAP(4)
         // The thread bests already hold every entry appended in this step: the chunk caches of publish_best need not
         // cover them yet.
+        seg_cur = min(b.seg_len, b.cap0); // (before publish_best's barrier, behind which warp 0 hands out pages)
         publish_best(cx, best, pw, split);
         {
-            // this step's entries -> the cached maxima of the chunks that received them
-            const int seg1 = min(b.seg_len, b.cap0);
-            seg_cur = seg1; // (nothing is appended before the next step's team C starts, two exchanges' barriers away)
-            for (int r = tid; r <= b.hot_n; r += nt) {
-                if (r == 0)
-                    merge_appended_apply(cx, 0, 0, seg0, seg1);
-                else {
-                    const int k = r - 1, l1 = min(b.hot_len[k], b.hot_cap);
-                    merge_appended_apply(cx, r, b.cap0 + k * b.hot_cap, b.hot_snap[k], l1);
-                    b.hot_len[k] = l1; // the region's fill becomes the next step's snapshot
-                    b.hot_snap[k] = l1;
+            // this step's entries -> the cached maxima of the pages that received them; then the hot logs' room for the
+            // next step (warp 0; nothing is appended before the next step's team C starts, two exchanges' barriers away)
+            if (wid == 0) {
+                const int seg1 = min(b.seg_len, b.cap0);
+                for (int r = lane; r <= b.hot_n; r += 32) {
+                    if (r == 0)
+                        merge_appended_apply(cx, 0, seg0, seg1);
+                    else {
+                        const int k = r - 1, l1 = min(b.hot_len[k], b.hot_np[k] << cx.cfg.chunk_log);
+                        merge_appended_apply(cx, r, b.hot_snap[k], l1);
+                        b.hot_len[k] = l1; // the log's fill becomes the next step's snapshot
+                        b.hot_snap[k] = l1;
+                    }
                 }
+                __syncwarp();
+                hot_grow(cx);
             }
         }
         if (tid == pub) { // (it has published; nobody touches these before the barrier inside the collect)
@@ -391,16 +387,22 @@ __device__ __forceinline__ void solve_own_kernel_body(const ProblemDesc *probs, 
         cx.ws = wss[group];
         cx.seg = cx.ws.fseg + (size_t)cx.rank * cx.ws.fseg_cap;
         cx.b = &bctx;
-        unsigned char *sp = smem;
+        unsigned char *sp = smem; // (page_cache_bytes)
+        const int n = cfg.nchunk_cap;
         cx.cb_score = (uint32_t *)sp;
-        sp += sizeof(uint32_t) * cfg.nchunk_cap;
+        sp += sizeof(uint32_t) * n;
         cx.cb_khi = (uint32_t *)sp;
-        sp += sizeof(uint32_t) * cfg.nchunk_cap;
+        sp += sizeof(uint32_t) * n;
         cx.cb_klo = (uint32_t *)sp;
-        sp += sizeof(uint32_t) * cfg.nchunk_cap;
-        cx.dirty_list = (int *)sp;
-        sp += sizeof(int) * cfg.nchunk_cap;
-        cx.cb_dirty = sp;
+        sp += sizeof(uint32_t) * n;
+        uint16_t *h = (uint16_t *)sp;
+        cx.dirty_list = h, h += n;
+        cx.pg_owner = h, h += n;
+        cx.pg_used = h, h += n;
+        cx.pg_slot = h, h += n;
+        cx.pg_free = h, h += n;
+        cx.hot_pg = h, h += DA_HOT_MAX * DA_HOT_PAGES;
+        cx.cb_dirty = (unsigned char *)h;
         OwnCtx &ox = oxs;
         ox.ws = ows[group];
         ox.lay = own_plan(cfg.nchunk_cap, n_out_max, e_cap_max, lcap, hlog, narrow).lay;

@@ -86,7 +86,7 @@ struct GroupWs {
     int *col_len;      // [n_out_max]
     int *col_k;        // [n_out_max] digits per column at to_solution time
     uint32_t *mod_step; // [e_cap_max] step at which an expression was last rewritten (lazy histogram purge)
-    FEnt *fseg;        // [G][fseg_cap]
+    FEnt *fseg;        // [G][fseg_cap]: each CTA's page pool
     uint4 *heap;       // [n_out_max][32 lanes][heap_lane_cap][2] to_solution scratch (lane-private)
     unsigned *barrier; // monotonically increasing arrive counter
     unsigned long long *xchg; // [2][G][4] stamped all-gather slots (barrier + payload in one round trip)
@@ -98,9 +98,19 @@ struct GroupWs {
 struct LaunchCfg {
     int G;          // CTAs per group
     int cpc;        // output columns per CTA in the adder-tree phase
-    int chunk_log;  // log2(histogram entries per argmax chunk)
-    int nchunk_cap; // chunk-cache slots per CTA
-    int accounting; // 1: exact live-histogram size every step (re-reads every chunk), for traces / counters
+    int chunk_log;  // log2(histogram entries per page; a page is also the unit of the argmax cache)
+    int nchunk_cap; // page slots per CTA (pages of the pool + 2)
+    int accounting; // 1: exact live-histogram size every step (re-reads every page), for traces / counters
 };
+
+// Hot logs of a CTA's histogram (the entries whose passive partner is one of its first DA_HOT_MAX owned expressions) and
+// the pages one of them may hold.
+#define DA_HOT_MAX 64
+#define DA_HOT_PAGES 64
+// Shared-memory bytes of the page caches of `slots` pages: cached maximum (3 x u32), dirty-list slot, owner, used-list
+// slot and entry, free-stack entry (u16 each), dirty flag (u8), and the page tables of the hot logs (u16).
+__host__ __device__ inline size_t page_cache_bytes(int slots) {
+    return (size_t)slots * 23 + 2 * (size_t)DA_HOT_MAX * DA_HOT_PAGES;
+}
 
 } // namespace da

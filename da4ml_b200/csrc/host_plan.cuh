@@ -31,7 +31,7 @@ struct PlanEnv {
 inline size_t own_plan_bytes(int nchunk_cap, int n_out_max, int e_cap_max, int lcap, int hlog, int narrow) {
     auto up = [](size_t b) { return (b + 15) & ~size_t(15); };
     const size_t words = (size_t)(n_out_max + 31) / 32;
-    size_t o = up((size_t)nchunk_cap * 17);
+    size_t o = up(page_cache_bytes(nchunk_cap));
     o += 3 * up(8 * (size_t)n_out_max) + 5 * up(4 * words) + up(4 * (size_t)((e_cap_max + 31) / 32)) + up(4 * (size_t)n_out_max) + up(2 * (size_t)n_out_max) + up(4 * ((size_t)n_out_max + 1));
     o += 2 * up((size_t)4 << hlog) + up((size_t)2 << hlog) + up((narrow ? 6 : 12) * (size_t)n_out_max * (size_t)lcap);
     return o;
@@ -40,7 +40,7 @@ inline size_t own_plan_bytes(int nchunk_cap, int n_out_max, int e_cap_max, int l
 // ---- launch plan ---------------------------------------------------------------------------------------------------
 struct LaunchPlan {
     LaunchCfg cfg;
-    long long max_fcap = 0; // histogram-segment entries per CTA
+    long long max_fcap = 0; // histogram-segment entries per CTA (pages x page size)
     int n_groups = 1;
     int lcap = 0, hlog = 12;       // rows per owner list in shared memory, log2 of the pair-counter hash table
     int nbits_max = 1, narrow = 0; // narrow: list rows of 6 bytes
@@ -55,14 +55,18 @@ inline LaunchPlan plan_for_group(const std::vector<PlanJob> &jobs, const PlanEnv
     LaunchPlan P;
     memset(&P.cfg, 0, sizeof(P.cfg));
     long long rows_target = 0, rows_hard = 0;
+    // The histogram segment of a CTA is a pool of pages; each page has a cache in shared memory (page_cache_bytes), so the
+    // pool has at most `slots` pages.  Small pages keep what a dead cached winner costs small (one page re-read).
+    const int slots = (int)((48 * 1024 - page_cache_bytes(0)) / 23) - 2;
+    const int page_log_max = 10; // (measured at the bench shape: a pool of 512-entry pages compacts and loses more)
+    long long fcap = 0;
     for (const PlanJob &j : jobs) {
-        // (half of a segment is the common log, half the hot regions; a log that is still 3/4 full after a compaction would
-        // compact every step, so the capacity is generous.  A job that needs more reports it and is retried with f_mul x 4.)
-        const long long fcap_total = (128 * j.d0 + 65536) * j.f_mul;
-        P.max_fcap = std::max(P.max_fcap, fcap_total / G + fcap_total / (2 * G) + 8192);
-        // ... and never small: with many CTAs per problem a CTA's share of the initial histogram plus what spills out of its
-        // (then tiny) hot regions must not keep the common log above its compaction threshold (12 MB per CTA at most)
-        P.max_fcap = std::max(P.max_fcap, std::min<long long>(768 * 1024, 16 * j.d0 + 65536) * j.f_mul);
+        // what the worst case would need (all pair counts ever created, half as much again for the dead ones), but no
+        // more than pages of 2^page_log_max entries give; and at least twice a CTA's share of the initial histogram (its
+        // upper bound) plus room for the first steps.  A job that needs more reports it and is retried with f_mul x 4.
+        const long long worst = (128 * j.d0 + 65536) / G * 3 / 2 + 8192;
+        const long long init = (long long)j.n_in * (j.n_in + 1) / 2 * (2 * j.nbits - 1) * 2 / G;
+        fcap = std::max(fcap, std::max(std::min(worst, (long long)slots << page_log_max), 2 * init + 65536) * j.f_mul);
         P.n_out_max = std::max(P.n_out_max, j.n_out);
         P.e_cap_max = std::max(P.e_cap_max, j.e_cap);
         P.nbits_max = std::max(P.nbits_max, j.nbits);
@@ -72,16 +76,18 @@ inline LaunchPlan plan_for_group(const std::vector<PlanJob> &jobs, const PlanEnv
         rows_hard = std::max(rows_hard, std::min<long long>(j.col_cap, (long long)j.list_mul * 2 * own_in + 64));
         P.pool_cap = std::max(P.pool_cap, ((long long)j.n_in * j.n_out + j.d0) / G * j.list_mul + j.n_out + 64);
     }
-    if (P.max_fcap >= (1LL << 27))
-        P.max_fcap = (1LL << 27) - 1;
     LaunchCfg &cfg = P.cfg;
     cfg.G = G;
     cfg.cpc = (P.n_out_max + G - 1) / G;
     cfg.accounting = env.accounting ? 1 : 0;
     cfg.chunk_log = 6;
-    while ((((P.max_fcap >> cfg.chunk_log) + 2) * 17) > 44 * 1024) // (small chunks: what a dead cached winner costs is one chunk re-read)
+    while ((fcap >> cfg.chunk_log) > slots)
         ++cfg.chunk_log;
-    cfg.nchunk_cap = (int)((P.max_fcap >> cfg.chunk_log) + 2);
+    long long pages = std::min<long long>(slots, (fcap + (1LL << cfg.chunk_log) - 1) >> cfg.chunk_log);
+    while (pages > 1 && (pages << cfg.chunk_log) >= (1LL << 27))
+        --pages;
+    P.max_fcap = pages << cfg.chunk_log;
+    cfg.nchunk_cap = (int)pages + 2;
     const long long budget = env.own_budget;
     P.narrow = (P.nbits_max <= 16 && (P.e_cap_max + G - 1) / G + 1 <= 65535) ? 1 : 0;
     // pair-counter hash table: as large as the target list capacity leaves room for (2^13 ... 2^11 counters)

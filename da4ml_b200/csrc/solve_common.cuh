@@ -107,24 +107,28 @@ __device__ __forceinline__ Best warp_best(Best b) {
 }
 
 
-#define DA_HOT_MAX 64
 // Block-level context kept in shared memory
 struct BlockCtx {
     Best warp_best[32];
     int warp_sum[32];
     int warp_st[32];
     Best chosen;       // pair selected for the current step (score==0 -> none)
-    int seg_len;       // entries (live + dead) in the common log of this CTA's histogram segment, [0, cap0)
-    // Hot regions (owner-partitioned kernel): the entries whose passive partner is one of the first hot_n inputs this CTA
-    // owns get a region of their own, [cap0 + k * hot_cap, +hot_cap).  Such an input is rewritten over and over, and every
-    // time ALL entries of its region die at once: the region is simply reset instead of re-reading the chunks they led.
-    int cap0, hot_n, hot_cap;
-    int hot_len[DA_HOT_MAX];  // entries of each region (may run past hot_cap while a step appends: readers clamp)
+    // This CTA's histogram segment is a pool of `pages` pages of 2^chunk_log entries.  The common log fills it from page 0
+    // upwards, [0, seg_len); the hot logs take single pages from its top downwards, [hot_top, pages), and give them back
+    // to a free stack.  A hot log holds the entries whose passive partner is one of the first hot_n expressions this CTA
+    // owns: such an expression is rewritten over and over, and every time ALL entries of its log die at once -- its pages
+    // are freed instead of re-reading them.  A hot log that cannot get a page spills into the common log.
+    int seg_len;       // entries (live + dead) in the common log, [0, cap0)
+    int cap0;          // room of the common log: hot_top pages
+    int pages, hot_top, n_used, n_free, hot_n;
+    int hot_room;      // entries one step can append to one hot log at most: a hot log keeps that much room ahead
+    int hot_len[DA_HOT_MAX];  // entries of each hot log (may run past its pages while a step appends: readers clamp)
     int hot_snap[DA_HOT_MAX]; // the same at the start of the step (what the argmax caches have to cover)
+    int hot_np[DA_HOT_MAX];   // pages each hot log holds
     Best pend[DA_HOT_MAX + 1]; // maximum of the entries appended to each log in the current step (0: the common log)
     int n_new;         // entries appended in the current step
     int live_old;      // live entries counted by the last full rescan (accounting mode)
-    int n_dirty;       // chunks to re-read in the current step
+    int n_dirty;       // pages to re-read in the current step
     int status;        // sticky error
     int list_max;      // longest column list seen by this CTA
     unsigned long long r_count;   // digit pairs enumerated by this CTA (all steps)
@@ -150,9 +154,13 @@ struct Ctx {
     FEnt *seg; // this CTA's histogram segment (global)
     // shared memory
     BlockCtx *b;
-    uint32_t *cb_score, *cb_khi, *cb_klo; // per-chunk cached maximum
+    uint32_t *cb_score, *cb_khi, *cb_klo; // per-page cached maximum
     unsigned char *cb_dirty;
-    int *dirty_list;
+    uint16_t *dirty_list;
+    uint16_t *pg_owner;           // hot page -> (hot log << 8) | its index in that log
+    uint16_t *pg_used, *pg_slot;  // the hot pages in use [0, n_used), and each one's position in that list
+    uint16_t *pg_free;            // free stack of hot pages [0, n_free)
+    uint16_t *hot_pg;             // [DA_HOT_MAX][DA_HOT_PAGES] the pages of each hot log, in order
 };
 
 // Barrier across the G CTAs of a group: monotonic counter, release on arrive / acquire on poll, split in
@@ -292,24 +300,28 @@ __device__ __forceinline__ void load_op(const ProblemDesc &p, uint32_t id, QInt 
         cx.b->t_last = _now;                                                   \
     }
 
-// Chunks of the segment in use, and the entries [lo, hi) of chunk c (empty when the chunk lies beyond its region's
-// fill).  `seg_len` = fill of the common log; the hot regions' fills come from their step-start snapshot.
-__device__ __forceinline__ int chunks_in_use(const Ctx &cx, int seg_len) {
+// Pages of the segment in use: the common log's pages [0, nc) (nc = common_pages(seg_len)), then the hot pages in use.
+// `seg_len` = fill of the common log; the hot logs' fills come from their step-start snapshot.
+__device__ __forceinline__ int common_pages(const Ctx &cx, int seg_len) { return (seg_len + (1 << cx.cfg.chunk_log) - 1) >> cx.cfg.chunk_log; }
+__device__ __forceinline__ int pages_in_use(const Ctx &cx, int nc) { return nc + cx.b->n_used; }
+__device__ __forceinline__ int page_at(const Ctx &cx, int i, int nc) { return i < nc ? i : (int)cx.pg_used[i - nc]; }
+// the entries [lo, hi) of page pg
+__device__ __forceinline__ void page_span(const Ctx &cx, int pg, int seg_len, int &lo, int &hi) {
     const BlockCtx &b = *cx.b;
     const int cl = cx.cfg.chunk_log;
-    return b.hot_n ? (b.cap0 + b.hot_n * b.hot_cap) >> cl : (seg_len + (1 << cl) - 1) >> cl;
-}
-__device__ __forceinline__ void chunk_span(const Ctx &cx, int c, int seg_len, int &lo, int &hi) {
-    const BlockCtx &b = *cx.b;
-    lo = c << cx.cfg.chunk_log;
-    const int end = lo + (1 << cx.cfg.chunk_log);
-    if (b.hot_n == 0 || lo < b.cap0)
-        hi = min(end, seg_len);
+    lo = pg << cl;
+    if (pg < b.hot_top)
+        hi = min(lo + (1 << cl), seg_len);
     else {
-        const int k = (lo - b.cap0) / b.hot_cap;
-        hi = k < b.hot_n ? min(end, b.cap0 + k * b.hot_cap + b.hot_snap[k]) : lo;
+        const int o = cx.pg_owner[pg];
+        hi = lo + min(1 << cl, b.hot_snap[o >> 8] - ((o & 255) << cl));
     }
     hi = max(hi, lo);
+}
+// position of entry v of log r (0: the common log, k + 1: hot log k) in the segment
+__device__ __forceinline__ int log_pos(const Ctx &cx, int r, int v) {
+    const int cl = cx.cfg.chunk_log;
+    return r == 0 ? v : ((int)cx.hot_pg[(r - 1) * DA_HOT_PAGES + (v >> cl)] << cl) + (v & ((1 << cl) - 1));
 }
 
 // Append one histogram entry (created at step `stamp`) to this CTA's segment and fold it into the
@@ -321,10 +333,10 @@ emit_entry(const ProblemDesc &p, const Ctx &cx, uint32_t lo, uint32_t hi, int sh
         return; // NaN score: can never be selected
     const uint64_t key = pack_key(lo, hi, shift, sub);
     int pos = -1;
-    if (hot >= 0) { // the passive partner's own region; when that is full the entry goes to the common log like any other
+    if (hot >= 0) { // the passive partner's own log; when its pages are full the entry goes to the common log like any other
         const int q = smem_add(&cx.b->hot_len[hot], 1);
-        if (q < cx.b->hot_cap)
-            pos = cx.b->cap0 + hot * cx.b->hot_cap + q;
+        if (q < (cx.b->hot_np[hot] << cx.cfg.chunk_log))
+            pos = log_pos(cx, hot + 1, q);
     }
     if (pos < 0) {
         pos = smem_add(&cx.b->seg_len, 1);
@@ -342,7 +354,7 @@ emit_entry(const ProblemDesc &p, const Ctx &cx, uint32_t lo, uint32_t hi, int sh
     e.w = (uint32_t)(key >> 32);
     cx.seg[pos] = e;
     if (mark_dirty) // (else the caller marks the chunks of everything it appended)
-        st_racy(&cx.cb_dirty[pos >> cx.cfg.chunk_log], (unsigned char)1); // this chunk's cached maximum does not cover the new entry yet
+        st_racy(&cx.cb_dirty[pos >> cx.cfg.chunk_log], (unsigned char)1); // this page's cached maximum does not cover the new entry yet
     if (score >= thresh) {
         Best c{score, e.w, e.z};
         if (best_gt(c, best))

@@ -71,9 +71,9 @@ __device__ __forceinline__ int rescan_range(const Ctx &cx, int lo, int hi, uint3
     return live;
 }
 
-// Bring every chunk cache up to date for the substitution (c0, c1): chunks whose cached winner touches c0/c1,
-// chunks that received appends, or all chunks (accounting / after compaction).  Block-wide.  A chunk is re-read by
-// one warp, or -- when few large chunks are dirty -- by several warps that each take a 256-entry-aligned part of it.
+// Bring every page cache up to date for the substitution (c0, c1): pages whose cached winner touches c0/c1, pages
+// that received appends, or all pages in use (accounting / after compaction).  Block-wide.  A page is re-read by one
+// warp, or -- when few large pages are dirty -- by several warps that each take a 256-entry-aligned part of it.
 #ifndef DA_SPLIT_RESCAN
 #define DA_SPLIT_RESCAN 1
 #endif
@@ -82,10 +82,11 @@ __device__ void refresh_chunks(const Ctx &cx, const Team &tm, int seg_len, uint3
     const int tid = tm.tid, nt = tm.nt, lane = tid & 31, wid = tid >> 5, nw = nt >> 5;
     BlockCtx &b = *cx.b;
     const int ch_log = cx.cfg.chunk_log, ch = 1 << ch_log;
-    const int nchunks = chunks_in_use(cx, seg_len);
-    for (int c = tid; c < nchunks; c += nt) {
+    const int nc = common_pages(cx, seg_len), npages = pages_in_use(cx, nc);
+    for (int i = tid; i < npages; i += nt) {
+        const int c = page_at(cx, i, nc);
         int lo_c, hi_c;
-        chunk_span(cx, c, seg_len, lo_c, hi_c);
+        page_span(cx, c, seg_len, lo_c, hi_c);
         if (hi_c <= lo_c)
             continue; // (nothing there: its cache is empty)
         bool d = all || cx.cb_dirty[c];
@@ -108,7 +109,7 @@ __device__ void refresh_chunks(const Ctx &cx, const Team &tm, int seg_len, uint3
         if (wid < nd * nparts) {
             const int i = wid / nparts, part = wid - i * nparts;
             int base, end;
-            chunk_span(cx, cx.dirty_list[i], seg_len, base, end);
+            page_span(cx, cx.dirty_list[i], seg_len, base, end);
             const int plen = ch / nparts;
             const int lo = base + part * plen;
             Best pb;
@@ -136,7 +137,7 @@ __device__ void refresh_chunks(const Ctx &cx, const Team &tm, int seg_len, uint3
         for (int i = wid; i < nd; i += nw) {
             const int chunk = cx.dirty_list[i];
             int base, end;
-            chunk_span(cx, chunk, seg_len, base, end);
+            page_span(cx, chunk, seg_len, base, end);
             Best v;
             live += rescan_range(cx, base, end, c0, c1, purge, thresh, v);
             if (lane == 0) {
@@ -158,16 +159,16 @@ __device__ void refresh_chunks(const Ctx &cx, const Team &tm, int seg_len, uint3
         b.n_dirty = 0;
 }
 
-// Entries [l0, l1) of one log (the common one or a hot region starting at `base`) were appended in this step: their
-// maximum is folded into the cached maximum of their chunk instead of re-reading the whole chunk next step (they are live by
-// construction).  Part 1 (one warp, any time after the entries were written): the maximum -> pend[r]; part 2 (one thread,
-// when nobody else touches the caches): pend[r] -> the chunk's cache.  Entries that straddle a chunk boundary, or land in a
-// chunk that is dirty anyway, leave their chunks dirty instead.
-__device__ __forceinline__ void merge_appended_scan(const Ctx &cx, int r, int base, int l0, int l1, uint32_t thresh) {
+// Entries [l0, l1) of log r (0: the common log, k + 1: hot log k) were appended in this step: their maximum is folded
+// into the cached maximum of their page instead of re-reading the whole page next step (they are live by construction).
+// Part 1 (one warp, any time after the entries were written): the maximum -> pend[r]; part 2 (one thread, when nobody
+// else touches the caches): pend[r] -> the page's cache.  Entries that straddle a page boundary, or land in a page that
+// is dirty anyway, leave their pages dirty instead.
+__device__ __forceinline__ void merge_appended_scan(const Ctx &cx, int r, int l0, int l1, uint32_t thresh) {
     const int lane = threadIdx.x & 31;
     Best best{0u, 0u, 0u};
-    for (int i = base + l0 + lane; i < base + l1; i += 32) {
-        const FEnt e = cx.seg[i];
+    for (int v = l0 + lane; v < l1; v += 32) {
+        const FEnt e = cx.seg[log_pos(cx, r, v)];
         if (e.x >= thresh) {
             const Best cand{e.x, e.w, e.z};
             if (best_gt(cand, best))
@@ -178,13 +179,13 @@ __device__ __forceinline__ void merge_appended_scan(const Ctx &cx, int r, int ba
     if (lane == 0)
         cx.b->pend[r] = best;
 }
-__device__ __forceinline__ void merge_appended_apply(const Ctx &cx, int r, int base, int l0, int l1) {
+__device__ __forceinline__ void merge_appended_apply(const Ctx &cx, int r, int l0, int l1) {
     if (l1 <= l0)
         return;
-    const int cl = cx.cfg.chunk_log, ca = (base + l0) >> cl, cb = (base + l1 - 1) >> cl;
-    if (ca != cb || cx.cb_dirty[ca]) {
-        for (int c = ca; c <= cb; ++c)
-            cx.cb_dirty[c] = 1;
+    const int cl = cx.cfg.chunk_log, ca = log_pos(cx, r, l0) >> cl;
+    if ((l0 >> cl) != ((l1 - 1) >> cl) || cx.cb_dirty[ca]) {
+        for (int v = l0 >> cl; v <= (l1 - 1) >> cl; ++v)
+            cx.cb_dirty[log_pos(cx, r, v << cl) >> cl] = 1;
         return;
     }
     const Best best = cx.b->pend[r], cur{cx.cb_score[ca], cx.cb_khi[ca], cx.cb_klo[ca]};
@@ -195,8 +196,91 @@ __device__ __forceinline__ void merge_appended_apply(const Ctx &cx, int r, int b
     }
 }
 
-// In-place compaction of this CTA's segment (drops dead entries; order is irrelevant), then every chunk cache
-// is rebuilt.  Tiles of 8 x blockDim entries: all reads of a tile complete before its survivors are written to
+// Warp 0, between steps: give every hot log the room one step can fill (hot_room entries beyond its fill) -- pages from
+// the free stack first, then from the top of the pool while the common log keeps at least twice its fill below.  A log
+// that gets no page spills into the common log until it does.
+__device__ void hot_grow(const Ctx &cx) {
+    BlockCtx &b = *cx.b;
+    const int lane = threadIdx.x & 31, cl = cx.cfg.chunk_log;
+    const int lim = (2 * b.seg_len + (1 << cl) - 1) >> cl;
+    for (int k0 = 0; k0 < b.hot_n; k0 += 32) {
+        const int k = k0 + lane;
+        int np = 0, need = 0;
+        if (k < b.hot_n) {
+            np = b.hot_np[k];
+            while (np + need < DA_HOT_PAGES && ((np + need) << cl) < b.hot_len[k] + b.hot_room)
+                ++need;
+        }
+        int incl = need;
+#pragma unroll
+        for (int off = 1; off < 32; off <<= 1) {
+            const int u = __shfl_up_sync(0xffffffffu, incl, off);
+            if (lane >= off)
+                incl += u;
+        }
+        const int total = __shfl_sync(0xffffffffu, incl, 31);
+        if (total == 0) // (warp-uniform)
+            continue;
+        const int n_free = b.n_free, top = b.hot_top, n_used = b.n_used;
+        const int from_stack = min(total, n_free), from_top = min(total - from_stack, max(0, top - lim));
+        for (int g = incl - need; g < incl && g < from_stack + from_top; ++g) {
+            const int pg = g < from_stack ? cx.pg_free[n_free - 1 - g] : top - 1 - (g - from_stack);
+            cx.pg_owner[pg] = (uint16_t)((k << 8) | np);
+            cx.hot_pg[k * DA_HOT_PAGES + np] = (uint16_t)pg;
+            cx.pg_used[n_used + g] = (uint16_t)pg;
+            cx.pg_slot[pg] = (uint16_t)(n_used + g);
+            ++np;
+        }
+        if (need)
+            b.hot_np[k] = np;
+        __syncwarp();
+        if (lane == 0) {
+            b.n_free = n_free - from_stack;
+            b.hot_top = top - from_top;
+            b.n_used = n_used + from_stack + from_top;
+            b.cap0 = b.hot_top << cl;
+        }
+        __syncwarp();
+    }
+}
+
+// Block-wide, at the start of a step (uniform over the CTA): the hot logs of `mask` (bit w: log k[w]) were rewritten --
+// every entry of theirs is dead.  Each keeps its first page, emptied, and returns the others to the free stack.
+__device__ void hot_free(const Ctx &cx, const int k[2], unsigned mask) {
+    BlockCtx &b = *cx.b;
+    const int tid = threadIdx.x, nt = blockDim.x;
+    for (int w = 0; w < 2; ++w) {
+        if (!((mask >> w) & 1u))
+            continue;
+        const int np = b.hot_np[k[w]];
+        for (int j = tid; j < np; j += nt) {
+            const int pg = cx.hot_pg[k[w] * DA_HOT_PAGES + j];
+            cx.cb_score[pg] = 0u;
+            cx.cb_khi[pg] = 0u;
+            cx.cb_klo[pg] = 0u;
+            cx.cb_dirty[pg] = 0;
+        }
+    }
+    __syncthreads();
+    if (tid == 0)
+        for (int w = 0; w < 2; ++w) {
+            if (!((mask >> w) & 1u))
+                continue;
+            const int np = b.hot_np[k[w]];
+            for (int j = 1; j < np; ++j) {
+                const int pg = cx.hot_pg[k[w] * DA_HOT_PAGES + j];
+                cx.pg_free[b.n_free++] = (uint16_t)pg;
+                const int s = cx.pg_slot[pg], m = cx.pg_used[--b.n_used]; // (swap-remove from the list in use)
+                cx.pg_used[s] = (uint16_t)m;
+                cx.pg_slot[m] = (uint16_t)s;
+            }
+            b.hot_np[k[w]] = min(np, 1);
+            b.hot_len[k[w]] = b.hot_snap[k[w]] = 0;
+        }
+}
+
+// In-place compaction of this CTA's common log (drops dead entries; order is irrelevant), then every page cache is
+// rebuilt.  Tiles of 8 x blockDim entries: all reads of a tile complete before its survivors are written to
 // positions that never pass the tile's end.
 __device__ __noinline__ void compact_segment(const Ctx &cx, uint32_t c0, uint32_t c1, bool purge, uint32_t thresh, long long *compactions) {
     const int tid = threadIdx.x, nt = blockDim.x, lane = tid & 31;
@@ -237,9 +321,9 @@ __device__ __noinline__ void compact_segment(const Ctx &cx, uint32_t c0, uint32_
         if (compactions)
             atomicAdd((unsigned long long *)compactions, 1ull);
     }
-    // every cached maximum of the common log referred to the old positions: forget them all (the chunks in use are
-    // rebuilt below; the hot regions did not move)
-    for (int c = tid; c < (b.hot_n ? b.cap0 >> cx.cfg.chunk_log : cx.cfg.nchunk_cap); c += nt) {
+    // every cached maximum of the common log referred to the old positions: forget them all (the pages in use are
+    // rebuilt below; the hot logs did not move)
+    for (int c = tid; c < common_pages(cx, len); c += nt) {
         cx.cb_score[c] = 0u;
         cx.cb_khi[c] = 0u;
         cx.cb_klo[c] = 0u;
@@ -252,14 +336,18 @@ __device__ __noinline__ void compact_segment(const Ctx &cx, uint32_t c0, uint32_
     __syncthreads();
 }
 
-// Block-reduce (thread bests + chunk caches) and publish this CTA's candidate through the exchange: warp `pw` reduces, its
-// lane 0 publishes (`fenced`: that thread has already executed the release fence, see xchg_publish).  The chunk caches
+// Block-reduce (thread bests + page caches) and publish this CTA's candidate through the exchange: warp `pw` reduces, its
+// lane 0 publishes (`fenced`: that thread has already executed the release fence, see xchg_publish).  The page caches
 // are only read here, so the caller may update them as soon as this returns.
 __device__ void publish_best(const Ctx &cx, Best best, int pw, bool fenced) {
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, nw = blockDim.x >> 5;
     BlockCtx &b = *cx.b;
-    const int nchunks = chunks_in_use(cx, b.seg_len);
-    for (int c = tid; c < nchunks; c += blockDim.x) {
+    const int nc = common_pages(cx, b.seg_len), npages = pages_in_use(cx, nc);
+    // free pages run short: ask the whole group to compact together (read before the barrier, behind which warp 0 hands
+    // out the next pages)
+    const bool want = b.seg_len > b.cap0 - (b.cap0 >> 2);
+    for (int i = tid; i < npages; i += blockDim.x) {
+        const int c = page_at(cx, i, nc);
         Best cand{cx.cb_score[c], cx.cb_khi[c], cx.cb_klo[c]};
         if (best_gt(cand, best))
             best = cand;
@@ -273,7 +361,6 @@ __device__ void publish_best(const Ctx &cx, Best best, int pw, bool fenced) {
         v = warp_best(v);
         if (lane == 0) {
             const int live = cx.cfg.accounting ? b.live_old + b.n_new : 0;
-            const bool want = b.seg_len > b.cap0 - (b.cap0 >> 2); // ask the whole group to compact together
             xchg_publish(cx, v, b.status, want, live, fenced);
         }
     }

@@ -44,8 +44,9 @@ int da4ml_cmvm_set_group_size(int ctas_per_problem);
  * without touching a device.  jobs: [n][8] int64 = {n_in, n_out, nbits, csd_digits, max_digits_per_column,
  * column_list_bound, f_mul, list_mul}; out: [12] int64 = {ctas_per_problem, concurrent_groups, columns_per_cta (adder
  * trees), list_rows_in_shared_memory, log2_chunk, chunk_slots, segment_entries_per_cta, log2_pair_counters,
- * dynamic_shared_bytes, shared_budget_bytes, narrow_rows (6-byte list rows), spill_rows}.  Diagnostic; the reference has
- * no counterpart. */
+ * dynamic_shared_bytes, shared_budget_bytes, narrow_rows (6-byte list rows), spill_rows}.  The histogram segment of a
+ * CTA is a pool of pages: log2_chunk is the page size, segment_entries_per_cta the pool, chunk_slots its pages + 2.
+ * Diagnostic; the reference has no counterpart. */
 int da4ml_cmvm_plan(const int64_t *jobs, int64_t n_jobs, int co_resident_ctas, int group_override, int64_t out[12]);
 
 /* Free the large device / pinned work buffers the library caches between calls (re-grown on demand; function-local
@@ -53,7 +54,7 @@ int da4ml_cmvm_plan(const int64_t *jobs, int64_t n_jobs, int co_resident_ctas, i
 int da4ml_cmvm_release(void);
 
 /* Exact work accounting (sum over iterations of the live histogram size, needed for the algorithmic-bytes
- * figure): when on, every iteration re-reads the whole histogram instead of only the chunks whose cached
+ * figure): when on, every iteration re-reads the whole histogram instead of only the pages whose cached
  * maximum was invalidated.  Results are identical; only the counters and the speed change.  Off by default;
  * implied by a trace request. */
 int da4ml_cmvm_set_accounting(int on);
