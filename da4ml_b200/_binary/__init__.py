@@ -10,7 +10,9 @@ The shared library is the product's only compute path; importing this module wit
 
 from __future__ import annotations
 
+import copy
 import ctypes as C
+from collections import namedtuple
 from pathlib import Path
 
 import numpy as np
@@ -43,6 +45,8 @@ _L.da4ml_cmvm_solve_batch.argtypes = [C.c_int64, C.POINTER(_f32p), _i64p, _i64p,
 _L.da4ml_cmvm_solve_batch_device.argtypes = [C.c_int64, C.POINTER(_vp), _i64p, _i64p, C.c_char_p, C.c_char_p, C.c_int, C.c_int, C.POINTER(_f32p), C.POINTER(_f32p), C.c_int, C.c_int, C.c_int, C.POINTER(_vp)]
 _L.da4ml_cmvm_solve_single.argtypes = [_f32p, C.c_int64, C.c_int64, C.c_char_p, _f32p, _f32p, C.c_int, C.c_int, _i32p, C.c_int64, C.POINTER(_vp)]
 _L.da4ml_cmvm_solve_sweep.argtypes = [_f32p, C.c_int64, C.c_int64, _f32p, _f32p, C.c_int, C.c_int, C.c_int64, C.POINTER(C.c_char_p), C.POINTER(C.c_char_p), _i32p, _i32p, _i32p, C.c_int, C.POINTER(_vp)]
+_L.da4ml_cmvm_solve_sweep_batch.argtypes = [C.c_int64, C.POINTER(_f32p), _i64p, _i64p, C.POINTER(_f32p), C.POINTER(_f32p), C.c_int, C.c_int, C.c_int64, C.POINTER(C.c_char_p),
+                                            C.POINTER(C.c_char_p), _i32p, _i32p, _i32p, C.c_int, C.POINTER(_vp)]
 _L.da4ml_sweep_counts.argtypes = [_vp, _i64p]
 _L.da4ml_sweep_profile.argtypes = [_vp, C.POINTER(C.c_double)]
 _L.da4ml_sweep_summary.argtypes = [_vp, _i64p, _f32p]
@@ -87,7 +91,7 @@ EXPORTED_SYMBOLS = [
     'da4ml_cmvm_csd_decompose', 'da4ml_cmvm_int_arr_to_csd', 'da4ml_cmvm_kernel_decompose',
     'da4ml_cmvm_get_lsb_loc', 'da4ml_cmvm_iceil_log2', 'da4ml_cmvm_cost_add', 'da4ml_dais_run',
     'da4ml_dais_program_load', 'da4ml_dais_program_info', 'da4ml_dais_program_run', 'da4ml_dais_program_run_stream',
-    'da4ml_dais_program_free', 'da4ml_dais_program_profile', 'da4ml_dais_program_dump', 'da4ml_cmvm_solve_sweep', 'da4ml_sweep_counts',
+    'da4ml_dais_program_free', 'da4ml_dais_program_profile', 'da4ml_dais_program_dump', 'da4ml_cmvm_solve_sweep', 'da4ml_cmvm_solve_sweep_batch', 'da4ml_sweep_counts',
     'da4ml_sweep_profile', 'da4ml_sweep_summary', 'da4ml_sweep_pipeline', 'da4ml_sweep_free', 'da4ml_sweep_front',
 ]  # fmt: skip
 
@@ -399,10 +403,14 @@ class SweepResult:
     ``cost`` (float32, summed over both stages in op order, the value the argmin uses), ``n_adders``, ``latency_min`` /
     ``latency_max`` (``Pipeline.latency``), ``n_ops0`` / ``n_ops1``, and the flags ``winner``, ``front``, ``kept`` (op
     tables available through ``raw`` / ``pipeline``).  ``front`` and ``winners`` are index arrays; ``winners[s]`` is set
-    ``s``'s result, what ``solve(kernel, **option_sets[s])`` returns."""
+    ``s``'s result, what ``solve(kernel, **option_sets[s])`` returns.
+
+    A result pickles (``torch.distributed`` gathers, multiprocessing, files): the copy holds the candidate arrays and the
+    op tables of the kept candidates, and no library handle, and answers every method as the original does."""
 
     def __init__(self, handle, kernel, option_sets, qintervals, latencies, adder_size, carry_size):
         self._h = handle
+        self._kept = None  # {candidate: RawPipeline} once detached from the library by pickling
         self.kernel, self.option_sets = kernel, option_sets
         self._call = dict(qintervals=qintervals, latencies=latencies, adder_size=adder_size, carry_size=carry_size)
         cnt = np.zeros(4, np.int64)
@@ -433,11 +441,28 @@ class SweepResult:
         if h:
             _L.da4ml_sweep_free(h)
 
+    def __getstate__(self):
+        st = {k: v for k, v in self.__dict__.items() if k != '_h'}
+        if self._h:
+            st['_kept'] = {int(i): self.raw(i) for i in np.flatnonzero(self.candidates['kept'])}
+        return st
+
+    def __setstate__(self, st):
+        self.__dict__.update(st)
+        self._h = None
+
     def raw(self, i: int) -> RawPipeline:
         """Candidate ``i`` as a ``RawPipeline``; ``ValueError`` when its op tables were not kept."""
-        h = _vp()
-        _check(_L.da4ml_sweep_pipeline(self._h, int(i), C.byref(h)))
-        return RawPipeline(h)
+        if self._h:
+            h = _vp()
+            _check(_L.da4ml_sweep_pipeline(self._h, int(i), C.byref(h)))
+            return RawPipeline(h)
+        i, n = int(i), len(self)  # (a pickled copy: the library's checks and messages)
+        if not 0 <= i < n:
+            raise ValueError(f'sweep_pipeline: candidate {i} is out of range [0, {n})')
+        if i not in self._kept:
+            raise ValueError(f'sweep_pipeline: the op tables of candidate {i} were not kept (only the winners and the front are, unless the sweep was run with keep_all)')
+        return copy.deepcopy(self._kept[i])
 
     def pipeline(self, i: int, types_module=None):
         return self.raw(i).to_pipeline(types_module)
@@ -450,33 +475,121 @@ class SweepResult:
                     search_all_decompose_dc=False, **self._call)
 
 
+def _for_matrix(i, f, *args):
+    try:
+        return f(*args)
+    except (TypeError, ValueError, RuntimeError) as e:
+        raise type(e)(f'matrix {i}: {e}') from None
+
+
+def solve_sweep_batch(kernels, option_sets, qintervals=None, latencies=None, adder_size=-1, carry_size=-1, keep_all=False) -> list[SweepResult]:
+    """Solve every matrix of ``kernels`` under every option set of ``option_sets`` in one GPU pass (a model's layers,
+    say): every pending ``solve_single`` of every candidate of every matrix runs in one launch per round.
+
+    ``qintervals`` / ``latencies`` are per-matrix lists, as for ``solve_batch_raw``.  The option sets and the cost model
+    (``adder_size``, ``carry_size``) are shared by all matrices, so costs of different matrices can be summed.  Result
+    ``p`` is what ``solve_sweep(kernels[p], option_sets, ...)`` returns (its ``profile`` is the whole call's).  If any set
+    fails on any matrix, the call raises ``solve``'s error and returns nothing."""
+    named = _for_matrix if len(kernels) > 1 else (lambda i, f, *args: f(*args))  # (a lone matrix needs no name)
+    ks = [named(i, _kernel_arg, k) for i, k in enumerate(kernels)]
+    n = len(ks)
+    sets = [dict(s) for s in option_sets]
+    for s in sets:
+        bad = set(s) - set(SWEEP_SET_DEFAULTS)
+        if bad:
+            raise TypeError(f'unsupported keys in a sweep option set: {sorted(bad)} (adder_size / carry_size are arguments of the sweep itself)')
+    for name, v in (('qintervals', qintervals), ('latencies', latencies)):
+        if v is not None and len(v) != n:
+            raise ValueError(f'expected {name} for {n} matrices, got {len(v)}')
+    qs = [named(i, _qint_arg, qintervals[i], ks[i].shape[0]) if qintervals is not None else None for i in range(n)]
+    ls = [named(i, _lat_arg, latencies[i], ks[i].shape[0]) if latencies is not None else None for i in range(n)]
+    if n == 0:
+        return []
+    full = [{**SWEEP_SET_DEFAULTS, **s} for s in sets]
+    m = len(full)
+    m0 = (C.c_char_p * max(m, 1))(*[str(s['method0']).encode() for s in full])
+    m1 = (C.c_char_p * max(m, 1))(*[str(s['method1']).encode() for s in full])
+    hdc = np.asarray([int(s['hard_dc']) for s in full] or [0], np.int32)
+    ddc = np.asarray([int(s['decompose_dc']) for s in full] or [0], np.int32)
+    sa = np.asarray([int(bool(s['search_all_decompose_dc'])) for s in full] or [0], np.int32)
+    kp = (_f32p * n)(*[_fp(k) for k in ks])
+    qp = (_f32p * n)(*[_fp(q) for q in qs])
+    lp = (_f32p * n)(*[_fp(l) for l in ls])
+    n_in = np.asarray([k.shape[0] for k in ks], np.int64)
+    n_out = np.asarray([k.shape[1] for k in ks], np.int64)
+    hs = (_vp * n)()
+    i32 = lambda a: a.ctypes.data_as(_i32p)  # noqa: E731
+    _check(_L.da4ml_cmvm_solve_sweep_batch(n, kp, _ip(n_in), _ip(n_out), qp, lp, int(adder_size), int(carry_size), m, m0, m1, i32(hdc), i32(ddc), i32(sa),
+                                           int(bool(keep_all)), hs))
+    return [SweepResult(_vp(h), k, [dict(s) for s in sets], None if q is None else [tuple(map(float, r)) for r in q], None if l is None else [float(v) for v in l],
+                        int(adder_size), int(carry_size)) for h, k, q, l in zip(hs, ks, qs, ls)]
+
+
 def solve_sweep(kernel, option_sets, qintervals=None, latencies=None, adder_size=-1, carry_size=-1, keep_all=False) -> SweepResult:
     """Solve one matrix under every option set of ``option_sets`` in one GPU pass.
 
     Each option set is a dict of ``solve`` keywords (``method0, method1, hard_dc, decompose_dc,
     search_all_decompose_dc``; missing keys take ``solve``'s defaults).  The intervals, latencies and the cost model
     (``adder_size``, ``carry_size``) are shared by all sets: costs under different cost models are not comparable.
-    Op tables come back for the winners and the front, or for every candidate with ``keep_all``."""
-    k = _kernel_arg(kernel)
-    sets = [dict(s) for s in option_sets]
-    for s in sets:
-        bad = set(s) - set(SWEEP_SET_DEFAULTS)
-        if bad:
-            raise TypeError(f'unsupported keys in a sweep option set: {sorted(bad)} (adder_size / carry_size are arguments of the sweep itself)')
-    q = _qint_arg(qintervals, k.shape[0])
-    l = _lat_arg(latencies, k.shape[0])
-    full = [{**SWEEP_SET_DEFAULTS, **s} for s in sets]
-    n = len(full)
-    m0 = (C.c_char_p * max(n, 1))(*[str(s['method0']).encode() for s in full])
-    m1 = (C.c_char_p * max(n, 1))(*[str(s['method1']).encode() for s in full])
-    hdc = np.asarray([int(s['hard_dc']) for s in full] or [0], np.int32)
-    ddc = np.asarray([int(s['decompose_dc']) for s in full] or [0], np.int32)
-    sa = np.asarray([int(bool(s['search_all_decompose_dc'])) for s in full] or [0], np.int32)
-    h = _vp()
-    i32 = lambda a: a.ctypes.data_as(_i32p)  # noqa: E731
-    _check(_L.da4ml_cmvm_solve_sweep(_fp(k), k.shape[0], k.shape[1], _fp(q), _fp(l), int(adder_size), int(carry_size), n, m0, m1, i32(hdc), i32(ddc), i32(sa),
-                                     int(bool(keep_all)), C.byref(h)))
-    return SweepResult(h, k, sets, None if q is None else [tuple(map(float, r)) for r in q], None if l is None else [float(v) for v in l], int(adder_size), int(carry_size))
+    Op tables come back for the winners and the front, or for every candidate with ``keep_all``.  The batch of one
+    matrix of ``solve_sweep_batch``."""
+    return solve_sweep_batch([kernel], option_sets, None if qintervals is None else [qintervals], None if latencies is None else [latencies], adder_size, carry_size,
+                             keep_all)[0]
+
+
+NetworkPoint = namedtuple('NetworkPoint', ['cost', 'latency', 'choice'])
+
+
+class NetworkFront:
+    """The cost / latency front of a chain of layers (``network_front``).  ``cost`` and ``latency`` are float32 arrays
+    sorted by ascending latency; ``choice[p, k]`` is the candidate of layer ``k``'s sweep that point ``p`` uses."""
+
+    def __init__(self, cost, latency, choice):
+        self.cost, self.latency, self.choice = cost, latency, choice
+
+    def __len__(self):
+        return len(self.cost)
+
+    def best(self, latency_budget) -> NetworkPoint:
+        """The cheapest point whose latency is at most ``latency_budget`` (the first of equal ones); ``ValueError`` when
+        every point is slower."""
+        ok = np.flatnonzero(self.latency.astype(np.float64) <= float(latency_budget))
+        if ok.size == 0:
+            raise ValueError(f'no design of the network meets a latency budget of {latency_budget} (the fastest has latency {float(self.latency[0])})')
+        p = int(ok[np.argmin(self.cost[ok])])
+        return NetworkPoint(float(self.cost[p]), float(self.latency[p]), tuple(int(c) for c in self.choice[p]))
+
+
+def network_front(sweeps) -> NetworkFront:
+    """Combine the sweeps of a chain of layers (``sweeps[k]`` of layer ``k``, in order) into the network's front.
+
+    A point takes one candidate per layer from that layer's ``front``; its cost and latency are the float32 sums, in
+    layer order, of the layers' ``cost`` and ``latency_max``.  The combinations are built layer by layer, in
+    lexicographic order of the per-layer choices, and pruned after each layer with the ``sweep_front`` rule (of exactly
+    equal points the first is kept).  Every chosen candidate is on its layer's front, so its op tables are kept.
+
+    Latency model: each layer is swept with its input latencies counted from its own inputs (zeros by default).  An op's
+    latency is max-plus monotone in its operands' latencies, so shifting every input of a layer by t shifts each of its
+    outputs by at most t; the sum of the chosen graphs' ``latency_max`` therefore bounds the chain's adder depth from
+    the network inputs.  Branching networks are not covered."""
+    sweeps = list(sweeps)
+    if not sweeps:
+        raise ValueError('network_front needs the sweep of at least one layer')
+    cost = lat = choice = None
+    for sw in sweeps:
+        f = np.asarray(sw.front, np.int64)
+        c = np.asarray(sw.candidates['cost'], np.float32)[f]
+        l = np.asarray(sw.candidates['latency_max'], np.float32)[f]
+        if choice is None:
+            cost, lat, choice = c, l, f[:, None]
+        else:  # every (point so far, front candidate) pair, in lexicographic order of the choices
+            cost = (cost[:, None] + c[None, :]).ravel()
+            lat = (lat[:, None] + l[None, :]).ravel()
+            choice = np.concatenate([np.repeat(choice, f.size, axis=0), np.tile(f, len(choice))[:, None]], axis=1)
+        keep = sweep_front(cost, lat)
+        cost, lat, choice = cost[keep], lat[keep], choice[keep]
+    order = np.argsort(lat, kind='stable')
+    return NetworkFront(cost[order], lat[order], choice[order])
 
 
 def csd_decompose(inp, center=True):
@@ -544,6 +657,7 @@ def cost_add(q0, q1, shift: int, sub: bool, adder_size: int, carry_size: int):
 
 
 __all__ = [
-    'solve', 'solve_batch', 'solve_raw', 'solve_batch_raw', 'solve_batch_device_raw', 'solve_single_raw', 'solve_sweep', 'SweepResult', 'sweep_front', 'csd_decompose', 'int_arr_to_csd',
+    'solve', 'solve_batch', 'solve_raw', 'solve_batch_raw', 'solve_batch_device_raw', 'solve_single_raw', 'solve_sweep', 'solve_sweep_batch', 'SweepResult', 'sweep_front',
+    'network_front', 'NetworkFront', 'NetworkPoint', 'csd_decompose', 'int_arr_to_csd',
     'kernel_decompose', 'get_lsb_loc', 'iceil_log2', 'cost_add', 'dais_interp_run', 'device_info', 'plan', 'set_stream', 'set_group_size', 'set_accounting',
 ]  # fmt: skip

@@ -435,15 +435,21 @@ int da4ml_cmvm_solve_single(
     });
 }
 
-// ---- sweep: one matrix under many option sets ----------------------------------------------------
-int da4ml_cmvm_solve_sweep(
-    const float *kernel, int64_t n_in, int64_t n_out, const float *qintervals, const float *latencies, int adder_size, int carry_size, int64_t n_sets,
-    const char *const *method0, const char *const *method1, const int32_t *hard_dc, const int32_t *decompose_dc, const int32_t *search_all, int keep_all,
-    da4ml_sweep_t **out
+// ---- sweep: many matrices under many option sets ---------------------------------------------------
+int da4ml_cmvm_solve_sweep_batch(
+    int64_t n_problems, const float *const *kernels, const int64_t *n_in, const int64_t *n_out, const float *const *qintervals,
+    const float *const *latencies, int adder_size, int carry_size, int64_t n_sets, const char *const *method0, const char *const *method1,
+    const int32_t *hard_dc, const int32_t *decompose_dc, const int32_t *search_all, int keep_all, da4ml_sweep_t **out
 ) {
     return guarded([&] {
-        if (!kernel || n_in <= 0 || n_out <= 0)
-            throw ApiError(DA4ML_E_INVALID, "solve_sweep: kernel must be a non-empty 2D array");
+        if (n_problems <= 0)
+            throw ApiError(DA4ML_E_INVALID, "solve_sweep: n_problems must be positive (got " + std::to_string(n_problems) + ")");
+        if (!kernels || !n_in || !n_out)
+            throw ApiError(DA4ML_E_INVALID, "solve_sweep: a kernel array is null");
+        for (int64_t p = 0; p < n_problems; ++p) // (a lone matrix needs no name)
+            if (!kernels[p] || n_in[p] <= 0 || n_out[p] <= 0)
+                throw ApiError(DA4ML_E_INVALID, n_problems == 1 ? std::string("solve_sweep: kernel must be a non-empty 2D array")
+                                                                : "solve_sweep: kernel " + std::to_string(p) + " must be a non-empty 2D array");
         if (n_sets <= 0)
             throw ApiError(DA4ML_E_INVALID, "solve_sweep: n_sets must be positive (got " + std::to_string(n_sets) + ")");
         if (!method0 || !method1 || !hard_dc || !decompose_dc || !search_all)
@@ -459,11 +465,24 @@ int da4ml_cmvm_solve_sweep(
             if (sets[s].method1 != "auto")
                 parse_method(sets[s].method1);
         }
-        auto sw = std::make_unique<SweepImpl>();
+        std::vector<SweepImpl> sweeps;
         std::vector<std::unique_ptr<PipelineImpl>> winners;
-        solve_many(1, &kernel, &n_in, &n_out, sets, &qintervals, &latencies, adder_size, carry_size, winners, false, sw.get(), keep_all != 0);
-        *out = new da4ml_sweep{std::move(sw)};
+        solve_many(n_problems, kernels, n_in, n_out, sets, qintervals, latencies, adder_size, carry_size, winners, false, &sweeps, keep_all != 0);
+        std::vector<std::unique_ptr<da4ml_sweep>> res((size_t)n_problems); // (all results exist before any is handed out)
+        for (int64_t p = 0; p < n_problems; ++p)
+            res[p].reset(new da4ml_sweep{std::make_unique<SweepImpl>(std::move(sweeps[p]))});
+        for (int64_t p = 0; p < n_problems; ++p)
+            out[p] = res[p].release();
     });
+}
+
+int da4ml_cmvm_solve_sweep(
+    const float *kernel, int64_t n_in, int64_t n_out, const float *qintervals, const float *latencies, int adder_size, int carry_size, int64_t n_sets,
+    const char *const *method0, const char *const *method1, const int32_t *hard_dc, const int32_t *decompose_dc, const int32_t *search_all, int keep_all,
+    da4ml_sweep_t **out
+) {
+    return da4ml_cmvm_solve_sweep_batch(1, &kernel, &n_in, &n_out, &qintervals, &latencies, adder_size, carry_size, n_sets, method0, method1, hard_dc,
+                                        decompose_dc, search_all, keep_all, out);
 }
 
 int da4ml_sweep_counts(const da4ml_sweep_t *s, int64_t out[4]) {

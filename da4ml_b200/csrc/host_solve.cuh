@@ -150,19 +150,20 @@ static float stage_max_latency(const StageResult &r) {
 }
 
 // Every problem is solved under every option set of `sets`.  out[problem * sets.size() + set] receives the winner, the
-// result of solve(W, **set).  With `sweep` (one problem only) every candidate is summarised there instead, and the op
-// tables of the winners and of the front (of every candidate with keep_all) are kept; `out` stays empty.
+// result of solve(W, **set).  With `sweeps` every problem's candidates are summarised in (*sweeps)[problem] instead, with
+// the front computed within the problem, and the op tables of the winners and of the front (of every candidate with
+// keep_all) are kept; `out` stays empty.
 static void solve_many(
     int64_t n_problems, const float *const *kernels, const int64_t *n_in, const int64_t *n_out, const std::vector<SolveOptions> &sets,
     const float *const *qints, const float *const *lats, int adder_size, int carry_size, std::vector<std::unique_ptr<PipelineImpl>> &out,
-    bool kernels_on_device = false, SweepImpl *sweep = nullptr, bool keep_all = false
+    bool kernels_on_device = false, std::vector<SweepImpl> *sweeps = nullptr, bool keep_all = false
 ) {
     init_device();
     g_out_arena2.reset();
     Timing tm;
     int64_t jobs_total = 0, jobs_run = 0;
     const int n_sets = (int)sets.size();
-    if (n_sets <= 0 || (sweep && n_problems != 1))
+    if (n_sets <= 0 || n_problems <= 0)
         throw ApiError(DA4ML_E_INVALID, "invalid argument");
     // validate methods up front (the reference throws from the worker, api.cc:231-240)
     for (const SolveOptions &o : sets) {
@@ -530,7 +531,7 @@ static void solve_many(
             w = (int)e;
     }
     // Only the op tables of what is returned leave the device.  A lone set's winner is used once and can be moved.
-    const bool move_out = n_sets == 1 && !sweep;
+    const bool move_out = n_sets == 1 && !sweeps;
     auto pipeline_of = [&](Candidate &c, bool move) {
         fetch_ops(c.job0.res);
         fetch_ops(c.job1.res);
@@ -548,7 +549,7 @@ static void solve_many(
         pl.jobs_total = jobs_total;
         pl.jobs_run = jobs_run;
     };
-    if (sweep) { // (summaries first: the winners below may be moved out of the candidates otherwise)
+    if (sweeps) { // (summaries first: the winners below may be moved out of the candidates otherwise)
         // Pipeline.latency reads ops[out_idx] of the last stage with Python indexing: a dead output (-1) reads the last op
         std::vector<float4> last_op(cands.size());
         for (size_t ci = 0; ci < cands.size(); ++ci) {
@@ -557,48 +558,59 @@ static void solve_many(
                 CK(cudaMemcpyAsync(&last_op[ci], r.d_q + (r.n_ops_dev - 1), sizeof(float4), cudaMemcpyDeviceToHost, g_stream));
         }
         CK(cudaStreamSynchronize(g_stream));
-        sweep->n_sets = n_sets;
-        sweep->n_solved = (int64_t)cands.size();
-        sweep->cands.assign(entries.size(), CandidateSummary());
-        std::vector<float> cost(entries.size()), lat_max(entries.size());
-        for (size_t e = 0; e < entries.size(); ++e) {
-            const Candidate &c = cands[entries[e].cand];
-            const StageResult &r0 = c.job0.res, &r1 = c.job1.res;
-            CandidateSummary &s = sweep->cands[e];
-            s.set = entries[e].set;
-            s.hard_dc = entries[e].hard_dc;
-            s.decompose_dc_start = entries[e].dc_start;
-            s.method0 = parse_method(c.method0);
-            s.method1 = parse_method(c.method1);
-            s.decompose_dc = c.decompose_dc;
-            s.cost = r1.cost_sum;
-            s.n_ops0 = r0.n_ops_dev;
-            s.n_ops1 = r1.n_ops_dev;
-            s.n_adders = (r0.n_ops_dev - r0.n_in) + (r1.n_ops_dev - r1.n_in); // (each stage's first n_in ops copy its inputs)
-            for (size_t k = 0; k < r1.out_idxs.size(); ++k) {
-                const float l = r1.out_idxs[k] >= 0 ? r1.out_q[k].w : last_op[entries[e].cand].w;
-                s.latency_min = k == 0 ? l : std::min(s.latency_min, l);
-                s.latency_max = k == 0 ? l : std::max(s.latency_max, l);
+        sweeps->clear();
+        sweeps->resize((size_t)n_problems);
+        // the entries of one problem are contiguous, in set order, then try order
+        for (size_t e0 = 0, e1 = 0; e0 < entries.size(); e0 = e1) {
+            const int pi = entries[e0].problem;
+            while (e1 < entries.size() && entries[e1].problem == pi)
+                ++e1;
+            SweepImpl &sw = (*sweeps)[pi];
+            const size_t n_e = e1 - e0;
+            sw.n_sets = n_sets;
+            sw.n_solved = (int64_t)probs[pi].cand.size();
+            sw.cands.assign(n_e, CandidateSummary());
+            std::vector<float> cost(n_e), lat_max(n_e);
+            for (size_t k = 0; k < n_e; ++k) {
+                const size_t e = e0 + k;
+                const Candidate &c = cands[entries[e].cand];
+                const StageResult &r0 = c.job0.res, &r1 = c.job1.res;
+                CandidateSummary &s = sw.cands[k];
+                s.set = entries[e].set;
+                s.hard_dc = entries[e].hard_dc;
+                s.decompose_dc_start = entries[e].dc_start;
+                s.method0 = parse_method(c.method0);
+                s.method1 = parse_method(c.method1);
+                s.decompose_dc = c.decompose_dc;
+                s.cost = r1.cost_sum;
+                s.n_ops0 = r0.n_ops_dev;
+                s.n_ops1 = r1.n_ops_dev;
+                s.n_adders = (r0.n_ops_dev - r0.n_in) + (r1.n_ops_dev - r1.n_in); // (each stage's first n_in ops copy its inputs)
+                for (size_t o = 0; o < r1.out_idxs.size(); ++o) {
+                    const float l = r1.out_idxs[o] >= 0 ? r1.out_q[o].w : last_op[entries[e].cand].w;
+                    s.latency_min = o == 0 ? l : std::min(s.latency_min, l);
+                    s.latency_max = o == 0 ? l : std::max(s.latency_max, l);
+                }
+                s.winner = win[(size_t)pi * n_sets + s.set] == (int)e;
+                cost[k] = s.cost;
+                lat_max[k] = s.latency_max;
             }
-            s.winner = win[(size_t)s.set] == (int)e;
-            cost[e] = s.cost;
-            lat_max[e] = s.latency_max;
-        }
-        std::vector<int8_t> front(entries.size());
-        pareto_front(cost.data(), lat_max.data(), (int64_t)entries.size(), front.data());
-        sweep->kept.resize(entries.size());
-        for (size_t e = 0; e < entries.size(); ++e) {
-            CandidateSummary &s = sweep->cands[e];
-            s.front = front[e] != 0;
-            if (keep_all || s.winner || s.front) {
-                sweep->kept[e] = pipeline_of(cands[entries[e].cand], false);
-                put_totals(*sweep->kept[e]);
+            std::vector<int8_t> front(n_e);
+            pareto_front(cost.data(), lat_max.data(), (int64_t)n_e, front.data());
+            sw.kept.resize(n_e);
+            for (size_t k = 0; k < n_e; ++k) {
+                CandidateSummary &s = sw.cands[k];
+                s.front = front[k] != 0;
+                if (keep_all || s.winner || s.front) {
+                    sw.kept[k] = pipeline_of(cands[entries[e0 + k].cand], false);
+                    put_totals(*sw.kept[k]);
+                }
             }
+            put_totals(sw.totals);
         }
-        put_totals(sweep->totals);
     }
     out.clear();
-    for (size_t k = 0; !sweep && k < win.size(); ++k) { // (a sweep hands its winners out through `kept`)
+    for (size_t k = 0; !sweeps && k < win.size(); ++k) { // (a sweep hands its winners out through `kept`)
         out.push_back(pipeline_of(cands[entries[win[k]].cand], move_out));
         put_totals(*out.back());
     }

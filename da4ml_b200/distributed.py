@@ -4,6 +4,7 @@ The path shards at the grain the reference itself parallelises: independent cons
 ``cmvm()`` call of a traced model, reference trace/fixed_variable_array.py:368-371) -- there is no exchange step
 between them, so no data-path collective is issued during the solve.  Each rank solves its share on its own
 GPU; the variable-length adder graphs are gathered afterwards with one ``all_gather_object`` (NCCL or gloo).
+``sweep_sharded`` does the same for option sweeps of many matrices.
 """
 
 from __future__ import annotations
@@ -66,3 +67,13 @@ def solve_sharded(kernels: Sequence[np.ndarray], solver: Callable | None = None,
     for part in gathered:
         merged.update(part)
     return [merged[i] for i in range(len(kernels))]
+
+
+def sweep_sharded(kernels: Sequence[np.ndarray], option_sets: Sequence[dict], group=None, gather: bool = True, solver: Callable | None = None, **kw):
+    """Sweep ``kernels`` under ``option_sets`` across the ranks of ``group``: ``solve_sharded``'s assignment and gather
+    around ``solver(list_of_kernels, option_sets, **kw) -> list_of_results`` (default ``solve_sweep_batch``, one GPU pass
+    per rank).  Per-matrix ``qintervals`` / ``latencies`` travel with their matrices; gathered ``SweepResult``s are
+    detached copies (see ``SweepResult``)."""
+    if solver is None:
+        from ._binary import solve_sweep_batch as solver  # noqa: PLC0415
+    return solve_sharded(kernels, solver=lambda ks, **o: solver(ks, option_sets, **o), group=group, gather=gather, **kw)

@@ -124,6 +124,20 @@ int da4ml_cmvm_solve_sweep(
     int carry_size, int64_t n_sets, const char *const *method0, const char *const *method1, const int32_t *hard_dc,
     const int32_t *decompose_dc, const int32_t *search_all, int keep_all, da4ml_sweep_t **out
 );
+/* Many matrices under the same option sets in one GPU pass (a model's layers, say): every pending solve_single of every
+ * candidate of every matrix runs in one launch per round.  Pointer arrays as for da4ml_cmvm_solve_batch; qintervals,
+ * latencies or any entry of them may be NULL.  The option sets and the cost model are shared by the call, so costs of
+ * different matrices can be summed.  out[p] is matrix p's result, exactly what da4ml_cmvm_solve_sweep returns for it
+ * alone (candidates, winners, front and kept op tables within the matrix, n_solved of the matrix); its profile is the
+ * whole call's.  Arguments are checked on the host before any device call and n_problems <= 0 gives DA4ML_E_INVALID.
+ * If any set fails on any matrix, the call fails with that error and no out[p] is written.  da4ml_cmvm_solve_sweep is
+ * the case n_problems = 1. */
+int da4ml_cmvm_solve_sweep_batch(
+    int64_t n_problems, const float *const *kernels, const int64_t *n_in, const int64_t *n_out, const float *const *qintervals,
+    const float *const *latencies, int adder_size, int carry_size, int64_t n_sets, const char *const *method0,
+    const char *const *method1, const int32_t *hard_dc, const int32_t *decompose_dc, const int32_t *search_all, int keep_all,
+    da4ml_sweep_t **out /* [n_problems] */
+);
 /* counts: {n_sets, n_candidates, n_kept (candidates with op tables), n_solved (distinct candidates solved)} */
 int da4ml_sweep_counts(const da4ml_sweep_t *s, int64_t out[4]);
 /* Profile of the sweep call, as da4ml_pipeline_profile: {device_ms, launches, solve_kernel_ms, solve_kernel_launches,
