@@ -28,7 +28,6 @@ __host__ __device__ inline OwnPlan own_plan(int nchunk_cap, int n_out_max, int e
         P.lay.D[r] = take(sizeof(uint2) * (size_t)n_out_max);
     for (int r = 0; r < 3; ++r)
         P.lay.B[r] = take(sizeof(uint32_t) * (size_t)words);
-    P.lay.A = take(sizeof(uint32_t) * (size_t)words);
     P.lay.pre = take(sizeof(uint32_t) * (size_t)words);
     P.lay.ver = take(sizeof(uint32_t) * (size_t)((e_cap_max + 31) / 32));
     P.lay.col_len = take(sizeof(int) * (size_t)n_out_max);
@@ -126,8 +125,9 @@ __device__ void solve_problem_own(const ProblemDesc &p, const Ctx &cx, const Own
     if (r0)
         atomicAdd(&b.r_count, r0);
     __syncthreads();
-    const unsigned long long r0_cta = b.r_count;
     if (tid == 0) {
+        atomicAdd((unsigned long long *)&p.result_meta[META_R0], b.r_count);
+        b.r_count = 0ull; // from here on: the digit pairs of the greedy steps
         b.seg_len = min(b.seg_len, b.cap0);
         b.n_new = 0;
     }
@@ -163,7 +163,8 @@ __device__ void solve_problem_own(const ProblemDesc &p, const Ctx &cx, const Own
     int t = 0;
     unsigned long long sum_f = 0;
     int status = b.scratch_i[1];
-    const long long t_start = clock64();
+    if (tid == 0)
+        b.t_start = clock64();
     while (status == ST_OK) {
         const Best ch = b.chosen;
         if (ch.score == 0u || p.method == M_DUMMY)
@@ -234,7 +235,7 @@ __device__ void solve_problem_own(const ProblemDesc &p, const Ctx &cx, const Own
         }
         best = Best{0u, 0u, 0u};
         if (in_c) {
-            // A. substitution in every column (redundantly on every CTA), B. the owners update their cells and lists,
+            // A. substitution in the columns of c0 / c1 (redundantly on every CTA), B. the owners update their cells and lists,
             // C. the recount appends this step's entries
             own_substitute(p, cx, ox, tm_c, c0, c1, shift, sub);
             DA_LAP(0)
@@ -245,13 +246,6 @@ __device__ void solve_problem_own(const ProblemDesc &p, const Ctx &cx, const Own
             if (!split && !compacting)
                 refresh_chunks(cx, tm_c, seg0, c0, c1, true, cx.cfg.accounting != 0, thresh);
             own_recount(p, cx, ox, tm_c, newid, stamp, thresh, best);
-            // maxima of the entries each log received in this step (their chunks' caches are updated behind the join)
-            for (int r = wid; r <= b.hot_n; r += nt_c >> 5) {
-                const int l0 = r == 0 ? seg0 : b.hot_snap[r - 1];
-                const int l1 = r == 0 ? min(b.seg_len, b.cap0) : min(b.hot_len[r - 1], b.hot_np[r - 1] << cx.cfg.chunk_log);
-                if (l1 > l0) // (uniform over the warp; most logs receive nothing in a step)
-                    merge_appended_scan(cx, r, l0, l1, thresh);
-            }
             DA_LAP(1)
         }
         else {
@@ -280,16 +274,32 @@ __device__ void solve_problem_own(const ProblemDesc &p, const Ctx &cx, const Own
         // cover them yet.
         seg_cur = min(b.seg_len, b.cap0); // (before publish_best's barrier, behind which warp 0 hands out pages)
         publish_best(cx, best, pw, split);
+        own_clear_rows(p, ox, team_all()); // (the rows were last read before the join)
         {
-            // this step's entries -> the cached maxima of the pages that received them; then the hot logs' room for the
-            // next step (warp 0; nothing is appended before the next step's team C starts, two exchanges' barriers away)
+            // While the exchange is in flight: the maxima of the entries each log received in this step (every warp but
+            // the exchange's takes some logs; only a log whose new entries lie in one page that is not dirty anyway needs
+            // it), then warp 0 folds them into the cached maxima of their pages and gives the hot logs their room for the
+            // next step (nothing is appended before the next step's team C starts, two exchanges' barriers away).
+            const int nm = nw > 1 ? nw - 1 : 1, cl = cx.cfg.chunk_log; // (the exchange's warp is the last one)
+            if (wid < nm) {
+                for (int r = wid; r <= b.hot_n; r += nm) {
+                    const int l0 = r == 0 ? seg0 : b.hot_snap[r - 1];
+                    const int l1 = r == 0 ? min(b.seg_len, b.cap0) : min(b.hot_len[r - 1], b.hot_np[r - 1] << cl);
+                    if (l1 > l0 && (l0 >> cl) == ((l1 - 1) >> cl) && !cx.cb_dirty[log_pos(cx, r, l0) >> cl]) // (uniform over the warp)
+                        merge_appended_scan(cx, r, l0, l1, thresh);
+                }
+                if (nm > 1)
+                    team_sync(Team{tid, 32 * nm, 4});
+                else
+                    __syncwarp();
+            }
             if (wid == 0) {
                 const int seg1 = min(b.seg_len, b.cap0);
                 for (int r = lane; r <= b.hot_n; r += 32) {
                     if (r == 0)
                         merge_appended_apply(cx, 0, seg0, seg1);
                     else {
-                        const int k = r - 1, l1 = min(b.hot_len[k], b.hot_np[k] << cx.cfg.chunk_log);
+                        const int k = r - 1, l1 = min(b.hot_len[k], b.hot_np[k] << cl);
                         merge_appended_apply(cx, r, b.hot_snap[k], l1);
                         b.hot_len[k] = l1; // the log's fill becomes the next step's snapshot
                         b.hot_snap[k] = l1;
@@ -315,7 +325,7 @@ __device__ void solve_problem_own(const ProblemDesc &p, const Ctx &cx, const Own
             long long *ms = &p.result_meta[META_MILESTONES + 9 * (31 - __clz(t / 250))]; // (diagnostic: where the time of a stage goes)
             for (int k = 0; k < 8; ++k)
                 ms[k] = b.phase[k];
-            ms[8] = clock64() - t_start;
+            ms[8] = clock64() - b.t_start;
 #ifdef DA_RECOUNT_PROF
             printf("  recount parts after %d steps (cumulative ms at 1.9 GHz): setup %.2f counting %.2f harvest %.2f\n", t, ob.xphase[0] / 1.9e6, ob.xphase[1] / 1.9e6, ob.xphase[2] / 1.9e6);
 #endif
@@ -334,8 +344,7 @@ __device__ void solve_problem_own(const ProblemDesc &p, const Ctx &cx, const Own
     if (tid == 0) {
         b.r_count += (unsigned long long)b.r_step;
         b.rescanned += (unsigned long long)b.rescan_step;
-        atomicAdd((unsigned long long *)&p.result_meta[META_SUM_R], b.r_count - r0_cta);
-        atomicAdd((unsigned long long *)&p.result_meta[META_R0], r0_cta);
+        atomicAdd((unsigned long long *)&p.result_meta[META_SUM_R], b.r_count);
         atomicAdd((unsigned long long *)&p.result_meta[META_RESCANNED], b.rescanned);
         atomicMax((long long *)&p.result_meta[META_LIST_MAX], (long long)b.list_max);
         for (int k = 0; k < 8; ++k)

@@ -32,7 +32,7 @@ inline size_t own_plan_bytes(int nchunk_cap, int n_out_max, int e_cap_max, int l
     auto up = [](size_t b) { return (b + 15) & ~size_t(15); };
     const size_t words = (size_t)(n_out_max + 31) / 32;
     size_t o = up(page_cache_bytes(nchunk_cap));
-    o += 3 * up(8 * (size_t)n_out_max) + 5 * up(4 * words) + up(4 * (size_t)((e_cap_max + 31) / 32)) + up(4 * (size_t)n_out_max) + up(2 * (size_t)n_out_max) + up(4 * ((size_t)n_out_max + 1));
+    o += 3 * up(8 * (size_t)n_out_max) + 4 * up(4 * words) + up(4 * (size_t)((e_cap_max + 31) / 32)) + up(4 * (size_t)n_out_max) + up(2 * (size_t)n_out_max) + up(4 * ((size_t)n_out_max + 1));
     o += 2 * up((size_t)4 << hlog) + up((size_t)2 << hlog) + up((narrow ? 6 : 12) * (size_t)n_out_max * (size_t)lcap);
     return o;
 }

@@ -138,6 +138,7 @@ struct BlockCtx {
     int scratch_i[4];
     long long phase[8];
     long long t_last;
+    long long t_start; // start of the greedy loop (thread 0; the milestones of the phase timers)
     long long poll_iters;
     long long peak[8];
     long long nslow[8];

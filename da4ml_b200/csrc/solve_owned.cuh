@@ -2,8 +2,8 @@
 //
 // Expression e is owned by CTA e mod G of its group.  Two views of the live digits are kept:
 //   * cells (global memory): per expression, the list of (column, P, N) of its digits.  Written by the owner, read by
-//     every CTA of the group when the expression is chosen: each CTA rebuilds the dense rows of c0 and c1 in shared
-//     memory and computes the substitution for all columns itself (update_expr, state_opr.cc:227-283).
+//     every CTA of the group when the expression is chosen: each CTA rebuilds the rows of c0 and c1 in shared memory
+//     and computes the substitution in their columns itself (update_expr, state_opr.cc:227-283).
 //   * owner lists (shared memory of the owner, private): for every output column the rows (e / G, P, N) of the owned
 //     expressions that have digits there.  The recount (update_stats, state_opr.cc:307-340) walks the lists of the
 //     columns the rewritten rows touch -- work proportional to the rows of those columns -- and counts digit pairs in
@@ -56,8 +56,7 @@ struct OwnBlock {
 // shared-memory layout of one CTA, as byte offsets into the dynamic shared memory (so that accesses compile to LDS / STS)
 struct OwnLayout {
     uint32_t D[3];    // uint2[n_out_max] dense rows of the rewritten expressions after the substitution (D[1] = new row for a self pair)
-    uint32_t B[3];    // uint32[words] their column bitmaps
-    uint32_t A;       // uint32[words] union of the three
+    uint32_t B[3];    // uint32[words] column bitmaps: B[0] / B[1] of c0 / c1 before the substitution, B[new] of the new row
     uint32_t pre;     // uint32[words] exclusive prefix of popc(B[new])
     uint32_t ver;     // uint32[ceil(e_cap / 32)] rewrite parity of every expression
     uint32_t col_len; // int[n_out_max] rows of each owner list
@@ -214,6 +213,12 @@ __device__ void own_init(const ProblemDesc &p, const Ctx &cx, const OwnCtx &ox) 
     uint32_t *ver = DA_SM(uint32_t, ox.lay.ver);
     for (int i = tid; i < (p.e_cap + 31) / 32; i += nt)
         ver[i] = 0u;
+    for (int o = tid; o < p.n_out; o += nt) // (own_substitute expects the rows zero outside the columns it writes)
+        for (int r = 0; r < 3; ++r)
+            DA_SM(uint2, ox.lay.D[r])[o] = make_uint2(0u, 0u);
+    for (int w = tid; w < (p.n_out + 31) >> 5; w += nt)
+        for (int r = 0; r < 3; ++r)
+            DA_SM(uint32_t, ox.lay.B[r])[w] = 0u;
     const int n_own = p.n_in > cx.rank ? (p.n_in - cx.rank + G - 1) / G : 0; // owned inputs: rank, rank + G, ...
     const int cap = ox.lay.lcap + ox.ws.ovf_cap;
     for (int o = wid; o < p.n_out; o += nw) {
@@ -275,108 +280,87 @@ __device__ void own_init(const ProblemDesc &p, const Ctx &cx, const OwnCtx &ox) 
     }
 }
 
-// ---- A. dense rows of c0 / c1 from their cells, the substitution in every column, bitmaps of the three new rows -----
+// ---- A. rows of c0 / c1 from their cells, the substitution in the columns where they have digits -------------------
+// Work and shared-memory traffic follow the cells of c0 and c1, not n_out: between steps D[0..2] and the bitmaps B[0..2]
+// are zero (own_clear_rows clears what a step set), so a row is rebuilt by writing its live cells only.  B[0] / B[1] mark
+// the columns where c0 / c1 have digits, B[new] those of the new row afterwards (for a self pair B[1] is the new row's).
+// The touched columns -- where c0 or c1 has digits, which are exactly the columns where one of the three rows has digits
+// afterwards -- are listed in tcol, in no particular order.
 __device__ void own_substitute(const ProblemDesc &p, const Ctx &cx, const OwnCtx &ox, const Team &tm, uint32_t c0, uint32_t c1, int shift, int sub) {
     DA_DYN_SHARED(da_smem);
     const int tid = tm.tid, nt = tm.nt, lane = tid & 31, wid = tid >> 5, nw = nt >> 5;
     const bool self = c0 == c1;
     uint2 *D0 = DA_SM(uint2, ox.lay.D[0]), *D1 = self ? D0 : DA_SM(uint2, ox.lay.D[1]), *Dn = DA_SM(uint2, ox.lay.D[self ? 1 : 2]);
     uint32_t *ver = DA_SM(uint32_t, ox.lay.ver);
-    // (the directory entries and the first cells are requested before the rows are cleared: their latency overlaps)
     const uint2 dir0 = __ldcg(&ox.ws.cell_dir[c0]);
-    const uint2 dir1 = self ? dir0 : __ldcg(&ox.ws.cell_dir[c1]);
+    const uint2 dir1 = self ? make_uint2(0u, 0u) : __ldcg(&ox.ws.cell_dir[c1]);
     const uint2 *pl0 = ox.ws.cell_pl[(ver[c0 >> 5] >> (c0 & 31)) & 1u];
     const uint2 *pl1 = ox.ws.cell_pl[(ver[c1 >> 5] >> (c1 & 31)) & 1u];
-    uint2 a0 = make_uint2(0u, 0u), a1 = make_uint2(0u, 0u);
-    uint32_t k0 = 0u, k1 = 0u;
-    if ((uint32_t)tid < dir0.y) {
-        a0 = __ldcg(&pl0[dir0.x + tid]);
-        k0 = __ldcg(&ox.ws.cell_col[dir0.x + tid]);
-    }
-    if (!self && (uint32_t)tid < dir1.y) {
-        a1 = __ldcg(&pl1[dir1.x + tid]);
-        k1 = __ldcg(&ox.ws.cell_col[dir1.x + tid]);
-    }
-    for (int o = tid; o < p.n_out; o += nt) {
-        DA_SM(uint2, ox.lay.D[0])[o] = make_uint2(0u, 0u);
-        DA_SM(uint2, ox.lay.D[1])[o] = make_uint2(0u, 0u);
-        DA_SM(uint2, ox.lay.D[2])[o] = make_uint2(0u, 0u);
+    const int n0 = (int)dir0.y, n = n0 + (int)dir1.y;
+    if (tid == 0)
+        ox.ob->n_tcol = 0;
+    for (int i = tid; i < n; i += nt) { // the cells of c0, then those of c1
+        const int r = i < n0 ? 0 : 1;
+        const uint32_t c = r == 0 ? dir0.x + (uint32_t)i : dir1.x + (uint32_t)(i - n0);
+        const uint32_t k = __ldcg(&ox.ws.cell_col[c]);
+        const uint2 a = __ldcg(&(r == 0 ? pl0 : pl1)[c]);
+        if ((a.x | a.y) == 0u)
+            continue; // a dead cell
+        DA_SM(uint2, ox.lay.D[r])[k] = a;
+        atomicOr(&DA_SM(uint32_t, ox.lay.B[r])[k >> 5], 1u << (k & 31));
     }
     team_sync(tm);
-    if ((uint32_t)tid < dir0.y)
-        D0[k0] = a0;
-    if (!self && (uint32_t)tid < dir1.y)
-        D1[k1] = a1;
-    for (uint32_t i = tid + nt; i < dir0.y; i += nt)
-        D0[__ldcg(&ox.ws.cell_col[dir0.x + i])] = __ldcg(&pl0[dir0.x + i]);
-    if (!self)
-        for (uint32_t i = tid + nt; i < dir1.y; i += nt)
-            D1[__ldcg(&ox.ws.cell_col[dir1.x + i])] = __ldcg(&pl1[dir1.x + i]);
-    team_sync(tm);
-    const int n_pad = (p.n_out + 31) & ~31;
-    for (int o0 = wid * 32; o0 < n_pad; o0 += nw * 32) {
-        const int o = o0 + lane;
-        uint32_t P0 = 0u, N0 = 0u, P1 = 0u, N1 = 0u, Pn = 0u, Nn = 0u;
-        if (o < p.n_out) {
-            const uint2 a = D0[o], c = D1[o];
-            P0 = a.x, N0 = a.y, P1 = c.x, N1 = c.y;
+    // a warp per bitmap word that c0 or c1 has digits in, a lane per column
+    const uint32_t *B0 = DA_SM(uint32_t, ox.lay.B[0]), *B1 = DA_SM(uint32_t, ox.lay.B[1]);
+    uint32_t *Bn = DA_SM(uint32_t, ox.lay.B[self ? 1 : 2]);
+    uint16_t *tcol = DA_SM(uint16_t, ox.lay.tcol);
+    const int words = (p.n_out + 31) >> 5;
+    for (int w = wid; w < words; w += nw) {
+        const uint32_t u = B0[w] | (self ? 0u : B1[w]);
+        if (u == 0u)
+            continue; // (uniform over the warp)
+        const int k = (w << 5) + lane;
+        uint32_t Pn = 0u, Nn = 0u;
+        if ((u >> lane) & 1u) {
+            const uint2 a0 = D0[k], a1 = D1[k];
+            uint32_t P0 = a0.x, N0 = a0.y, P1 = a1.x, N1 = a1.y;
             if ((P0 | N0) != 0u && (P1 | N1) != 0u)
                 substitute_planes(P0, N0, P1, N1, self, shift, sub, p.nbits, Pn, Nn);
-            D0[o] = make_uint2(P0, N0);
+            D0[k] = make_uint2(P0, N0);
             if (!self)
-                D1[o] = make_uint2(P1, N1);
-            Dn[o] = make_uint2(Pn, Nn);
+                D1[k] = make_uint2(P1, N1);
+            Dn[k] = make_uint2(Pn, Nn);
         }
-        const unsigned b0 = __ballot_sync(0xffffffffu, (P0 | N0) != 0u);
-        const unsigned b1 = __ballot_sync(0xffffffffu, (P1 | N1) != 0u);
         const unsigned bn = __ballot_sync(0xffffffffu, (Pn | Nn) != 0u);
+        int base = 0;
         if (lane == 0) {
-            const int w = o0 >> 5;
-            DA_SM(uint32_t, ox.lay.B[0])[w] = b0;
-            if (!self)
-                DA_SM(uint32_t, ox.lay.B[1])[w] = b1;
-            DA_SM(uint32_t, ox.lay.B[self ? 1 : 2])[w] = bn;
-            DA_SM(uint32_t, ox.lay.A)[w] = b0 | b1 | bn;
+            Bn[w] = bn;
+            base = smem_add(&ox.ob->n_tcol, __popc(u));
         }
+        base = __shfl_sync(0xffffffffu, base, 0);
+        if ((u >> lane) & 1u)
+            tcol[base + __popc(u & ((1u << lane) - 1u))] = (uint16_t)k;
+    }
+    if (tid == 0) { // this CTA's view of the versions: c0 and c1 have now been rewritten once more (everybody read the old ones above)
+        ver[c0 >> 5] ^= 1u << (c0 & 31);
+        if (!self)
+            ver[c1 >> 5] ^= 1u << (c1 & 31);
     }
     team_sync(tm);
-    if (wid == 0) {
-        // exclusive prefix over the new row's bitmap words (cell positions of the new expression) and the compact list
-        // of touched columns; this CTA's view of the versions: c0 and c1 have now been rewritten once more (everybody
-        // read the old ones above)
-        const uint32_t *Bn = DA_SM(uint32_t, ox.lay.B[self ? 1 : 2]), *A = DA_SM(uint32_t, ox.lay.A);
-        uint32_t *pre = DA_SM(uint32_t, ox.lay.pre);
-        uint16_t *tcol = DA_SM(uint16_t, ox.lay.tcol);
-        const int words = (p.n_out + 31) >> 5;
-        int acc = 0, nt_col = 0;
-        for (int w0 = 0; w0 < words; w0 += 32) {
-            const int w = w0 + lane;
-            const uint32_t bw = w < words ? Bn[w] : 0u, aw = w < words ? A[w] : 0u;
-            int cn = __popc(bw), ca = __popc(aw);
-            int in = cn, ia = ca;
-#pragma unroll
-            for (int off = 1; off < 32; off <<= 1) {
-                const int vn = __shfl_up_sync(0xffffffffu, in, off), va = __shfl_up_sync(0xffffffffu, ia, off);
-                if (lane >= off)
-                    in += vn, ia += va;
-            }
-            if (w < words)
-                pre[w] = (uint32_t)(acc + in - cn);
-            int pos = nt_col + ia - ca;
-            for (uint32_t m = aw; m; m &= m - 1)
-                tcol[pos++] = (uint16_t)((w << 5) + __ffs(m) - 1);
-            acc += __shfl_sync(0xffffffffu, in, 31);
-            nt_col += __shfl_sync(0xffffffffu, ia, 31);
-        }
-        if (lane == 0) {
-            ox.ob->new_cells = acc;
-            ox.ob->n_tcol = nt_col;
-            ver[c0 >> 5] ^= 1u << (c0 & 31);
-            if (!self)
-                ver[c1 >> 5] ^= 1u << (c1 & 31);
-        }
+}
+// end of the step (any time after the recount's last read of the rows): D[0..2] and B[0..2] back to zero
+__device__ void own_clear_rows(const ProblemDesc &p, const OwnCtx &ox, const Team &tm) {
+    DA_DYN_SHARED(da_smem);
+    const uint16_t *tcol = DA_SM(uint16_t, ox.lay.tcol);
+    const int n_tcol = ox.ob->n_tcol;
+    for (int i = tm.tid; i < n_tcol; i += tm.nt) {
+        const int o = tcol[i];
+        for (int r = 0; r < 3; ++r)
+            DA_SM(uint2, ox.lay.D[r])[o] = make_uint2(0u, 0u);
     }
-    team_sync(tm);
+    for (int w = tm.tid; w < (p.n_out + 31) >> 5; w += tm.nt)
+        for (int r = 0; r < 3; ++r)
+            DA_SM(uint32_t, ox.lay.B[r])[w] = 0u;
 }
 
 // ---- B. the owners write the rewritten rows back (cells + owner lists) and create the new expression -------------------
@@ -389,6 +373,30 @@ __device__ void own_update(const ProblemDesc &p, const Ctx &cx, const OwnCtx &ox
     const bool own0 = (int)(c0 % (uint32_t)G) == cx.rank, own1 = !self && (int)(c1 % (uint32_t)G) == cx.rank, ownn = (int)(newid % (uint32_t)G) == cx.rank;
     if (!(own0 || own1 || ownn))
         return; // (uniform over the CTA)
+    if (ownn && tid < 32) {
+        // exclusive prefix over the new row's bitmap words: its cells are laid out in column order
+        const int lane = tid;
+        const uint32_t *Bn = DA_SM(uint32_t, ox.lay.B[self ? 1 : 2]);
+        uint32_t *pre = DA_SM(uint32_t, ox.lay.pre);
+        const int words = (p.n_out + 31) >> 5;
+        int acc = 0;
+        for (int w0 = 0; w0 < words; w0 += 32) {
+            const int w = w0 + lane;
+            const int cn = w < words ? __popc(Bn[w]) : 0;
+            int in = cn;
+#pragma unroll
+            for (int off = 1; off < 32; off <<= 1) {
+                const int v = __shfl_up_sync(0xffffffffu, in, off);
+                if (lane >= off)
+                    in += v;
+            }
+            if (w < words)
+                pre[w] = (uint32_t)(acc + in - cn);
+            acc += __shfl_sync(0xffffffffu, in, 31);
+        }
+        if (lane == 0)
+            ox.ob->new_cells = acc;
+    }
     for (int r = 0; r < (self ? 1 : 2); ++r) {
         if (r == 1)
             team_sync(tm); // (uniform) the two rows of one column are rewritten one after the other
@@ -427,7 +435,9 @@ __device__ void own_update(const ProblemDesc &p, const Ctx &cx, const OwnCtx &ox
         const size_t pool = (size_t)cx.rank * ox.ws.pool_cap;
         const uint32_t jn = newid / (uint32_t)G;
         const int cap = ox.lay.lcap + ox.ws.ovf_cap;
-        for (int o = tid; o < p.n_out; o += nt) {
+        const uint16_t *tcol = DA_SM(uint16_t, ox.lay.tcol);
+        for (int i = tid; i < ox.ob->n_tcol; i += nt) {
+            const int o = tcol[i];
             const uint2 v = D[o];
             if ((v.x | v.y) == 0u)
                 continue;
