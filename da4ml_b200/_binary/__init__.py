@@ -475,11 +475,20 @@ class SweepResult:
                     search_all_decompose_dc=False, **self._call)
 
 
-def _for_matrix(i, f, *args):
+def _prefixed(tag, f, *args, **kw):
     try:
-        return f(*args)
+        return f(*args, **kw)
     except (TypeError, ValueError, RuntimeError) as e:
-        raise type(e)(f'matrix {i}: {e}') from None
+        raise type(e)(f'{tag}: {e}') from None
+
+
+def _sweep_sets(option_sets) -> list[dict]:
+    sets = [dict(s) for s in option_sets]
+    for s in sets:
+        bad = set(s) - set(SWEEP_SET_DEFAULTS)
+        if bad:
+            raise TypeError(f'unsupported keys in a sweep option set: {sorted(bad)} (adder_size / carry_size are arguments of the sweep itself)')
+    return sets
 
 
 def solve_sweep_batch(kernels, option_sets, qintervals=None, latencies=None, adder_size=-1, carry_size=-1, keep_all=False) -> list[SweepResult]:
@@ -490,14 +499,10 @@ def solve_sweep_batch(kernels, option_sets, qintervals=None, latencies=None, add
     (``adder_size``, ``carry_size``) are shared by all matrices, so costs of different matrices can be summed.  Result
     ``p`` is what ``solve_sweep(kernels[p], option_sets, ...)`` returns (its ``profile`` is the whole call's).  If any set
     fails on any matrix, the call raises ``solve``'s error and returns nothing."""
-    named = _for_matrix if len(kernels) > 1 else (lambda i, f, *args: f(*args))  # (a lone matrix needs no name)
+    named = (lambda i, f, *args: _prefixed(f'matrix {i}', f, *args)) if len(kernels) > 1 else (lambda i, f, *args: f(*args))  # (a lone matrix needs no name)
     ks = [named(i, _kernel_arg, k) for i, k in enumerate(kernels)]
     n = len(ks)
-    sets = [dict(s) for s in option_sets]
-    for s in sets:
-        bad = set(s) - set(SWEEP_SET_DEFAULTS)
-        if bad:
-            raise TypeError(f'unsupported keys in a sweep option set: {sorted(bad)} (adder_size / carry_size are arguments of the sweep itself)')
+    sets = _sweep_sets(option_sets)
     for name, v in (('qintervals', qintervals), ('latencies', latencies)):
         if v is not None and len(v) != n:
             raise ValueError(f'expected {name} for {n} matrices, got {len(v)}')
@@ -592,6 +597,142 @@ def network_front(sweeps) -> NetworkFront:
     return NetworkFront(cost[order], lat[order], choice[order])
 
 
+def _out_latencies(raw) -> np.ndarray:
+    """Latency of each output of a result (float32, ``CombLogic.out_latency`` of its last stage): the op latency at each
+    ``out_idx``, and 0.0 for a column with ``out_idx == -1`` (a constant zero)."""
+    last = raw.stages[-1]
+    idx = np.asarray(last['out_idxs'], np.int64)
+    lat = np.asarray(last['ops_f'], np.float32).reshape(-1, 5)[:, 3]
+    out = np.zeros(idx.size, np.float32)
+    out[idx >= 0] = lat[idx[idx >= 0]]
+    return out
+
+
+class ChainFront(NetworkFront):
+    """The cost / latency front of a chain of layers, each solved under the output latencies of the one before it
+    (``chain_front``).  ``cost`` and ``latency`` are float32 arrays sorted by ascending latency; ``choice[p, k]`` is the
+    candidate that point ``p`` takes at layer ``k``, an index into the sweep of that layer under the point's own input
+    latencies.  ``best(latency_budget)`` is ``NetworkFront.best``.  ``profile`` holds the sweeps' launches, device time
+    and jobs, in total and per layer (``layers[k]``: input-latency states, candidates, points kept, ...).
+
+    Only host arrays are held (each point's designs are ``RawPipeline`` copies), so a front pickles as it is."""
+
+    def __init__(self, cost, latency, choice, raws, calls, profile):
+        super().__init__(cost, latency, choice)
+        self._raws, self._calls, self.profile = raws, calls, profile
+
+    def raw(self, p: int, k: int) -> RawPipeline:
+        """Layer ``k``'s design in point ``p``."""
+        return copy.deepcopy(self._raws[p][k])
+
+    def pipelines(self, p: int, types_module=None) -> list:
+        """Point ``p``'s designs as one ``Pipeline`` per layer."""
+        return [r.to_pipeline(types_module) for r in self._raws[p]]
+
+    def reference_calls(self, p: int) -> list[dict]:
+        """Per layer, the keywords of the ``solve(kernels[k], **kw)`` call that returns layer ``k``'s design in point
+        ``p``: the candidate's options, the layer's ``qintervals`` and its input ``latencies`` as Python floats (for
+        ``k > 0``, the output latencies of the point's design of layer ``k - 1``)."""
+        return copy.deepcopy(self._calls[p])
+
+
+def _chain_layer(points, state_of, sweeps, state_lats):
+    """Extend the points of the layers so far by the next layer and prune.  ``points`` is ``None`` at layer 0, else
+    ``(cost, lat, choice, outs, raws, calls)``; ``state_of[p]`` is the index of point ``p``'s input-latency state in
+    ``sweeps`` and ``state_lats`` (lists of Python floats); at layer 0 there is one state and ``state_of == [0]``.
+    Parents are taken in order and each is extended by every ``front`` candidate of its state's sweep, in candidate
+    order; cost is the float32 sum in layer order, latency the new design's ``latency_max``; then the ``sweep_front``
+    rule.  ``outs[p]`` are the output latencies of point ``p``'s last design."""
+    fronts = [np.asarray(sw.front, np.int64) for sw in sweeps]
+    f_cost = [np.asarray(sw.candidates['cost'], np.float32)[f] for sw, f in zip(sweeps, fronts)]
+    f_lat = [np.asarray(sw.candidates['latency_max'], np.float32)[f] for sw, f in zip(sweeps, fronts)]
+    par = np.concatenate([np.full(fronts[s].size, p, np.int64) for p, s in enumerate(state_of)])
+    sidx = np.concatenate([np.full(fronts[s].size, s, np.int64) for s in state_of])
+    cand = np.concatenate([fronts[s] for s in state_of])
+    cost = np.concatenate([f_cost[s] for s in state_of])
+    lat = np.concatenate([f_lat[s] for s in state_of])
+    if points is not None:
+        cost = points[0][par] + cost
+    keep = sweep_front(cost, lat)
+    par, sidx, cand, cost, lat = par[keep], sidx[keep], cand[keep], cost[keep], lat[keep]
+    choice = cand[:, None] if points is None else np.concatenate([points[2][par], cand[:, None]], axis=1)
+    designs = {}  # (state, candidate) -> (RawPipeline, solve() keywords, output latencies), shared by the points using it
+    raws, calls, outs = [], [], []
+    for p, s, i in zip(par.tolist(), sidx.tolist(), cand.tolist()):
+        if (s, i) not in designs:
+            r = sweeps[s].raw(i)
+            designs[s, i] = (r, {**sweeps[s].reference_call(i), 'latencies': state_lats[s]}, _out_latencies(r))
+        r, call, o = designs[s, i]
+        raws.append([r] if points is None else [*points[4][p], r])
+        calls.append([call] if points is None else [*points[5][p], call])
+        outs.append(o)
+    return cost, lat, choice, outs, raws, calls
+
+
+def chain_front(kernels, option_sets, qintervals=None, latencies=None, adder_size=-1, carry_size=-1, solver=None) -> ChainFront:
+    """The cost / latency front of a chain of layers, each layer solved under the output latencies of the design chosen
+    for the layer before it, as a traced model's matmuls are: every reported design is what
+    ``solve(kernels[k], **front.reference_calls(p)[k])`` returns, and every reported cost and latency is the chain's own.
+
+    ``kernels[k]`` is layer ``k``'s constant matrix (``kernels[k].shape[1] == kernels[k + 1].shape[0]``).
+    ``option_sets`` and the cost model (``adder_size``, ``carry_size``) are those of ``solve_sweep`` and the same for
+    every layer.  ``qintervals`` is ``None`` or one entry per layer: ``None`` (``solve``'s default) or that layer's input
+    intervals, e.g. those of the quantizer in front of it; intervals are not carried over from a layer's outputs.
+    ``latencies`` are layer 0's input latencies (default zeros).
+
+    Search: layer 0 is swept once, and its ``front`` candidates are the first points.  At each later layer a point's
+    input-latency state is the output latencies of its last design (``Pipeline.out_latencies``; 0.0 for a constant-zero
+    output); points whose states are equal as float32 share one problem, and all the layer's states go into one
+    ``solver`` call (``solve_sweep_batch``: one GPU pass per layer).  Each point is extended by every ``front`` candidate
+    of its state's sweep; its cost is the float32 sum of the designs' costs in layer order, and its latency the new
+    design's ``latency_max``, which already contains the upstream latency.  The points are pruned after each layer with
+    the ``sweep_front`` rule, and the result is sorted by ascending latency.
+
+    Latency model: latency is the solver's op latency.  Activations between layers add none, as ``relu`` and ``wrap`` in
+    the tracer keep their input's latency, and ``latency_cutoff > 0`` pipelining is not modelled.  The front is the front
+    of the chains explored: the solver is not monotone in its input latencies, so pruning partial chains on (cost,
+    ``latency_max``) is a heuristic and a pruned chain could have led to a better design.  What is reported is exact.
+
+    Limits: a layer's states all run in one call, and their op tables stay on the device until that call ends; if they do
+    not fit (``DA4ML_E_CAPACITY``), or any set fails on any state, the call raises that layer's error prefixed with
+    ``layer k: `` and returns nothing.  Branching networks are not covered.  ``solver(kernels, option_sets, **kw)`` stands
+    in for ``solve_sweep_batch`` (same keywords and results)."""
+    ks = [_prefixed(f'layer {k}', _kernel_arg, W) for k, W in enumerate(kernels)]
+    if not ks:
+        raise ValueError('chain_front needs at least one layer')
+    for k in range(1, len(ks)):
+        if ks[k - 1].shape[1] != ks[k].shape[0]:
+            raise ValueError(f'layer {k - 1} has {ks[k - 1].shape[1]} outputs but layer {k} has {ks[k].shape[0]} inputs')
+    sets = _sweep_sets(option_sets)
+    if qintervals is not None and len(qintervals) != len(ks):
+        raise ValueError(f'expected qintervals for {len(ks)} layers, got {len(qintervals)}')
+    qs = [None if qintervals is None else _prefixed(f'layer {k}', _qint_arg, qintervals[k], W.shape[0]) for k, W in enumerate(ks)]
+    qs = [None if q is None else [tuple(map(float, r)) for r in q] for q in qs]
+    l0 = _prefixed('layer 0', _lat_arg, latencies, ks[0].shape[0])
+    states = [np.zeros(ks[0].shape[0], np.float32) if l0 is None else l0]
+    solver = solve_sweep_batch if solver is None else solver
+    prof = dict(launches=0, device_ms=0.0, jobs_run=0, jobs_total=0, layers=[])
+    points, state_of = None, np.zeros(1, np.int64)
+    for k, W in enumerate(ks):
+        if k > 0:  # one state per distinct output-latency vector, in order of first use
+            index = {}
+            state_of = np.asarray([index.setdefault(o.tobytes(), len(index)) for o in points[3]], np.int64)
+            states = [np.frombuffer(b, np.float32) for b in index]
+        n, lats = len(states), [[float(v) for v in s] for s in states]
+        sweeps = _prefixed(f'layer {k}', solver, [W] * n, sets, qintervals=[qs[k]] * n, latencies=lats, adder_size=int(adder_size), carry_size=int(carry_size))
+        points = _chain_layer(points, state_of, sweeps, lats)
+        p0 = sweeps[0].profile  # (the whole call's)
+        layer = dict(states=n, candidates=sum(len(sw.candidates['cost']) for sw in sweeps), points=len(points[0]),
+                     **{key: p0[key] for key in ('launches', 'device_ms', 'jobs_run', 'jobs_total')})
+        prof['layers'].append(layer)
+        for key in ('launches', 'device_ms', 'jobs_run', 'jobs_total'):
+            prof[key] += layer[key]
+        del sweeps  # (the designs are copied out: free the handles before the next layer's call)
+    cost, lat, choice, _, raws, calls = points
+    order = np.argsort(lat, kind='stable')
+    return ChainFront(cost[order], lat[order], choice[order], [raws[p] for p in order], [calls[p] for p in order], prof)
+
+
 def csd_decompose(inp, center=True):
     """(csd int8[n_in,n_out,N], shift0 int8[n_in], shift1 int8[n_out])  (bindings.cc:63-103)."""
     k = _kernel_arg(inp)
@@ -658,6 +799,6 @@ def cost_add(q0, q1, shift: int, sub: bool, adder_size: int, carry_size: int):
 
 __all__ = [
     'solve', 'solve_batch', 'solve_raw', 'solve_batch_raw', 'solve_batch_device_raw', 'solve_single_raw', 'solve_sweep', 'solve_sweep_batch', 'SweepResult', 'sweep_front',
-    'network_front', 'NetworkFront', 'NetworkPoint', 'csd_decompose', 'int_arr_to_csd',
+    'network_front', 'NetworkFront', 'NetworkPoint', 'chain_front', 'ChainFront', 'csd_decompose', 'int_arr_to_csd',
     'kernel_decompose', 'get_lsb_loc', 'iceil_log2', 'cost_add', 'dais_interp_run', 'device_info', 'plan', 'set_stream', 'set_group_size', 'set_accounting',
 ]  # fmt: skip

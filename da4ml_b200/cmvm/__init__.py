@@ -2,12 +2,13 @@
 (reference ``src/da4ml/cmvm/__init__.py``: ``solve``, ``kernel_decompose``, ``QInterval``, ``Op``, ``CombLogic`` and the
 ``solver_options_t`` keyword bundle that tracing code splats into ``solve``).  ``solve_batch`` / ``solve_calls`` are the
 GPU-side additions for many independent matrices, ``solve_sweep`` for one matrix under many option sets,
-``solve_sweep_batch`` for many matrices under many option sets and ``network_front`` for the cheapest per-layer choice of a
-chain of layers under a latency budget."""
+``solve_sweep_batch`` for many matrices under many option sets, ``network_front`` for the cheapest per-layer choice of a
+chain of layers under a latency budget, and ``chain_front`` for the same with each layer solved under the output latencies
+of the design before it (the designs and latencies a traced model gets)."""
 
 from typing import TypedDict
 
-from .._binary import NetworkFront, SweepResult, kernel_decompose, network_front, solve, solve_batch, solve_sweep, solve_sweep_batch
+from .._binary import ChainFront, NetworkFront, SweepResult, chain_front, kernel_decompose, network_front, solve, solve_batch, solve_sweep, solve_sweep_batch
 from ..batching import CmvmCall, SolveBatcher, solve_calls
 from ..types import CombLogic, Op, Pipeline, QInterval
 
@@ -28,4 +29,4 @@ solver_options_t = TypedDict(
     total=False,
 )
 
-__all__ = ['solve', 'solve_batch', 'solve_sweep', 'solve_sweep_batch', 'SweepResult', 'network_front', 'NetworkFront', 'solve_calls', 'CmvmCall', 'SolveBatcher', 'kernel_decompose', 'QInterval', 'Op', 'CombLogic', 'Pipeline', 'solver_options_t']
+__all__ = ['solve', 'solve_batch', 'solve_sweep', 'solve_sweep_batch', 'SweepResult', 'network_front', 'NetworkFront', 'chain_front', 'ChainFront', 'solve_calls', 'CmvmCall', 'SolveBatcher', 'kernel_decompose', 'QInterval', 'Op', 'CombLogic', 'Pipeline', 'solver_options_t']
