@@ -44,9 +44,13 @@ _L.da4ml_cmvm_solve.argtypes = [_f32p, C.c_int64, C.c_int64, C.c_char_p, C.c_cha
 _L.da4ml_cmvm_solve_batch.argtypes = [C.c_int64, C.POINTER(_f32p), _i64p, _i64p, C.c_char_p, C.c_char_p, C.c_int, C.c_int, C.POINTER(_f32p), C.POINTER(_f32p), C.c_int, C.c_int, C.c_int, C.POINTER(_vp)]
 _L.da4ml_cmvm_solve_batch_device.argtypes = [C.c_int64, C.POINTER(_vp), _i64p, _i64p, C.c_char_p, C.c_char_p, C.c_int, C.c_int, C.POINTER(_f32p), C.POINTER(_f32p), C.c_int, C.c_int, C.c_int, C.POINTER(_vp)]
 _L.da4ml_cmvm_solve_single.argtypes = [_f32p, C.c_int64, C.c_int64, C.c_char_p, _f32p, _f32p, C.c_int, C.c_int, _i32p, C.c_int64, C.POINTER(_vp)]
+_L.da4ml_cmvm_solve_seeded.argtypes = [_f32p, C.c_int64, C.c_int64, C.c_char_p, C.c_char_p, C.c_int, C.c_int, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_uint64, C.POINTER(_vp)]
+_L.da4ml_cmvm_solve_single_seeded.argtypes = [_f32p, C.c_int64, C.c_int64, C.c_char_p, _f32p, _f32p, C.c_int, C.c_int, _i32p, C.c_int64, C.c_uint64, C.POINTER(_vp)]
 _L.da4ml_cmvm_solve_sweep.argtypes = [_f32p, C.c_int64, C.c_int64, _f32p, _f32p, C.c_int, C.c_int, C.c_int64, C.POINTER(C.c_char_p), C.POINTER(C.c_char_p), _i32p, _i32p, _i32p, C.c_int, C.POINTER(_vp)]
 _L.da4ml_cmvm_solve_sweep_batch.argtypes = [C.c_int64, C.POINTER(_f32p), _i64p, _i64p, C.POINTER(_f32p), C.POINTER(_f32p), C.c_int, C.c_int, C.c_int64, C.POINTER(C.c_char_p),
                                             C.POINTER(C.c_char_p), _i32p, _i32p, _i32p, C.c_int, C.POINTER(_vp)]
+_L.da4ml_cmvm_solve_sweep_batch_seeded.argtypes = [C.c_int64, C.POINTER(_f32p), _i64p, _i64p, C.POINTER(_f32p), C.POINTER(_f32p), C.c_int, C.c_int, C.c_int64,
+                                                   C.POINTER(C.c_char_p), C.POINTER(C.c_char_p), _i32p, _i32p, _i32p, C.POINTER(C.c_uint64), C.c_int, C.POINTER(_vp)]
 _L.da4ml_sweep_counts.argtypes = [_vp, _i64p]
 _L.da4ml_sweep_profile.argtypes = [_vp, C.POINTER(C.c_double)]
 _L.da4ml_sweep_summary.argtypes = [_vp, _i64p, _f32p]
@@ -93,6 +97,7 @@ EXPORTED_SYMBOLS = [
     'da4ml_dais_program_load', 'da4ml_dais_program_info', 'da4ml_dais_program_run', 'da4ml_dais_program_run_stream',
     'da4ml_dais_program_free', 'da4ml_dais_program_profile', 'da4ml_dais_program_dump', 'da4ml_cmvm_solve_sweep', 'da4ml_cmvm_solve_sweep_batch', 'da4ml_sweep_counts',
     'da4ml_sweep_profile', 'da4ml_sweep_summary', 'da4ml_sweep_pipeline', 'da4ml_sweep_free', 'da4ml_sweep_front',
+    'da4ml_cmvm_solve_seeded', 'da4ml_cmvm_solve_single_seeded', 'da4ml_cmvm_solve_sweep_batch_seeded',
 ]  # fmt: skip
 
 COUNTER_NAMES = ['status', 'n_ops', 'T', 'sum_F', 'sum_R', 'F0', 'R0', 'D_final', 'F_max', 'compactions', 'D0', 'n_bits', 'group_ctas',
@@ -185,6 +190,29 @@ def _qint_arg(qintervals, n_in):
     if q.shape[0] != n_in:
         raise ValueError(f'expected {n_in} qintervals, got {q.shape[0]}')
     return q
+
+
+def _seed_arg(seed) -> int:
+    # a tie-break seed is an unsigned 64-bit integer (see solve); checked before any device call
+    if isinstance(seed, bool) or not isinstance(seed, (int, np.integer)):
+        raise TypeError(f'seed must be an integer, got {type(seed).__name__}')
+    s = int(seed)
+    if not 0 <= s < 2**64:
+        raise ValueError(f'seed must be in [0, 2**64), got {s}')
+    return s
+
+
+def tb_mask(seed) -> int:
+    """The tie-break mask of ``seed``: 0 for seed 0, else ``splitmix64(seed) & (2**36 - 1)`` (the id0, sub and shift bits
+    of the packed pair key).  Host restatement of the kernel's ``tb_mask`` (cmvm_num.cuh), for tests and tools."""
+    s = _seed_arg(seed)
+    if s == 0:
+        return 0
+    m = (1 << 64) - 1
+    x = (s + 0x9E3779B97F4A7C15) & m
+    x = ((x ^ (x >> 30)) * 0xBF58476D1CE4E5B9) & m
+    x = ((x ^ (x >> 27)) * 0x94D049BB133111EB) & m
+    return (x ^ (x >> 31)) & ((1 << 36) - 1)
 
 
 def _lat_arg(latencies, n_in):
@@ -313,19 +341,26 @@ class RawPipeline:
 
 
 def solve_raw(kernel, method0='wmc', method1='auto', hard_dc=-1, decompose_dc=-2, qintervals=None, latencies=None,
-              adder_size=-1, carry_size=-1, search_all_decompose_dc=True) -> RawPipeline:
+              adder_size=-1, carry_size=-1, search_all_decompose_dc=True, seed=0) -> RawPipeline:
     k = _kernel_arg(kernel)
     q = _qint_arg(qintervals, k.shape[0])
     l = _lat_arg(latencies, k.shape[0])
+    s = _seed_arg(seed)
     h = _vp()
-    _check(_L.da4ml_cmvm_solve(_fp(k), k.shape[0], k.shape[1], method0.encode(), method1.encode(), hard_dc, decompose_dc, _fp(q), _fp(l), adder_size, carry_size, int(bool(search_all_decompose_dc)), C.byref(h)))
+    _check(_L.da4ml_cmvm_solve_seeded(_fp(k), k.shape[0], k.shape[1], method0.encode(), method1.encode(), hard_dc, decompose_dc, _fp(q), _fp(l), adder_size, carry_size,
+                                      int(bool(search_all_decompose_dc)), s, C.byref(h)))  # fmt: skip
     return RawPipeline(h)
 
 
 def solve(kernel, method0='wmc', method1='auto', hard_dc=-1, decompose_dc=-2, qintervals=None, latencies=None,
-          adder_size=-1, carry_size=-1, search_all_decompose_dc=True):
-    """``da4ml._binary.cmvm_bin.solve`` (bindings.cc:235-248): returns a ``Pipeline`` of two ``CombLogic`` stages."""
-    return solve_raw(kernel, method0, method1, hard_dc, decompose_dc, qintervals, latencies, adder_size, carry_size, search_all_decompose_dc).to_pipeline()
+          adder_size=-1, carry_size=-1, search_all_decompose_dc=True, seed=0):
+    """``da4ml._binary.cmvm_bin.solve`` (bindings.cc:235-248): returns a ``Pipeline`` of two ``CombLogic`` stages.
+
+    ``seed`` (this library's extension, an integer in [0, 2**64)) picks the tie-break order of the greedy pair selection:
+    among pairs of equal score the one whose packed key XOR ``tb_mask(seed)`` is largest.  Seed 0 is the reference's
+    order, so ``seed=0`` gives the reference's result; another seed is an equally valid greedy run whose graph may cost
+    more or less.  ``solve_best_of`` keeps the cheapest of many seeds."""
+    return solve_raw(kernel, method0, method1, hard_dc, decompose_dc, qintervals, latencies, adder_size, carry_size, search_all_decompose_dc, seed).to_pipeline()
 
 
 def solve_batch_raw(kernels, method0='wmc', method1='auto', hard_dc=-1, decompose_dc=-2, qintervals=None, latencies=None,
@@ -364,20 +399,23 @@ def solve_batch(kernels, **kw):
     return [r.to_pipeline() for r in solve_batch_raw(kernels, **kw)]
 
 
-def solve_single_raw(kernel, method='wmc', qintervals=None, latencies=None, adder_size=-1, carry_size=-1, trace_cap=0):
-    """One CSE stage (reference ``solve_single``, cmvm_core.cc:227).  Returns (RawPipeline, trace[n,5] or None)."""
+def solve_single_raw(kernel, method='wmc', qintervals=None, latencies=None, adder_size=-1, carry_size=-1, trace_cap=0, seed=0):
+    """One CSE stage (reference ``solve_single``, cmvm_core.cc:227).  Returns (RawPipeline, trace[n,5] or None).
+    ``seed``: the tie-break order of ``solve``."""
     k = _kernel_arg(kernel)
     q = _qint_arg(qintervals, k.shape[0])
     l = _lat_arg(latencies, k.shape[0])
+    s = _seed_arg(seed)
     tr = np.zeros((max(trace_cap, 1), 5), np.int32)
     h = _vp()
-    _check(_L.da4ml_cmvm_solve_single(_fp(k), k.shape[0], k.shape[1], method.encode(), _fp(q), _fp(l), adder_size, carry_size, tr.ctypes.data_as(_i32p) if trace_cap > 0 else None, trace_cap, C.byref(h)))
+    _check(_L.da4ml_cmvm_solve_single_seeded(_fp(k), k.shape[0], k.shape[1], method.encode(), _fp(q), _fp(l), adder_size, carry_size,
+                                             tr.ctypes.data_as(_i32p) if trace_cap > 0 else None, trace_cap, s, C.byref(h)))  # fmt: skip
     raw = RawPipeline(h)
     return raw, (tr[: min(trace_cap, raw.counters[0]['T'])] if trace_cap > 0 else None)
 
 
 METHODS = ['mc', 'mc-dc', 'mc-pdc', 'wmc', 'wmc-dc', 'wmc-pdc', 'dummy']  # the library's method codes
-SWEEP_SET_DEFAULTS = dict(method0='wmc', method1='auto', hard_dc=-1, decompose_dc=-2, search_all_decompose_dc=True)  # as solve()
+SWEEP_SET_DEFAULTS = dict(method0='wmc', method1='auto', hard_dc=-1, decompose_dc=-2, search_all_decompose_dc=True, seed=0)  # as solve()
 _SWEEP_INT_FIELDS = ['set', 'hard_dc', 'decompose_dc_start', 'method0', 'method1', 'decompose_dc', 'n_adders', 'n_ops0', 'n_ops1', 'winner', 'front', 'kept']
 _SWEEP_FLOAT_FIELDS = ['cost', 'latency_min', 'latency_max']
 
@@ -468,11 +506,16 @@ class SweepResult:
         return self.raw(i).to_pipeline(types_module)
 
     def reference_call(self, i: int) -> dict:
-        """Keyword arguments of the ``solve(kernel, **kw)`` call whose result candidate ``i`` is."""
+        """Keyword arguments of the ``solve(kernel, **kw)`` call whose result candidate ``i`` is.  A candidate of a set with
+        a non-zero ``seed`` gets a ``seed`` keyword: that call is one of this library's ``solve``, which the reference's
+        has no counterpart for."""
         c = self.candidates
         s = {**SWEEP_SET_DEFAULTS, **self.option_sets[int(c['set'][i])]}
-        return dict(method0=s['method0'], method1=s['method1'], hard_dc=int(c['hard_dc'][i]), decompose_dc=int(c['decompose_dc_start'][i]),
+        call = dict(method0=s['method0'], method1=s['method1'], hard_dc=int(c['hard_dc'][i]), decompose_dc=int(c['decompose_dc_start'][i]),
                     search_all_decompose_dc=False, **self._call)
+        if int(s['seed']):
+            call['seed'] = int(s['seed'])
+        return call
 
 
 def _prefixed(tag, f, *args, **kw):
@@ -488,6 +531,8 @@ def _sweep_sets(option_sets) -> list[dict]:
         bad = set(s) - set(SWEEP_SET_DEFAULTS)
         if bad:
             raise TypeError(f'unsupported keys in a sweep option set: {sorted(bad)} (adder_size / carry_size are arguments of the sweep itself)')
+        if 'seed' in s:
+            s['seed'] = _seed_arg(s['seed'])
     return sets
 
 
@@ -517,6 +562,7 @@ def solve_sweep_batch(kernels, option_sets, qintervals=None, latencies=None, add
     hdc = np.asarray([int(s['hard_dc']) for s in full] or [0], np.int32)
     ddc = np.asarray([int(s['decompose_dc']) for s in full] or [0], np.int32)
     sa = np.asarray([int(bool(s['search_all_decompose_dc'])) for s in full] or [0], np.int32)
+    sd = (C.c_uint64 * max(m, 1))(*[int(s['seed']) for s in full])
     kp = (_f32p * n)(*[_fp(k) for k in ks])
     qp = (_f32p * n)(*[_fp(q) for q in qs])
     lp = (_f32p * n)(*[_fp(l) for l in ls])
@@ -524,8 +570,8 @@ def solve_sweep_batch(kernels, option_sets, qintervals=None, latencies=None, add
     n_out = np.asarray([k.shape[1] for k in ks], np.int64)
     hs = (_vp * n)()
     i32 = lambda a: a.ctypes.data_as(_i32p)  # noqa: E731
-    _check(_L.da4ml_cmvm_solve_sweep_batch(n, kp, _ip(n_in), _ip(n_out), qp, lp, int(adder_size), int(carry_size), m, m0, m1, i32(hdc), i32(ddc), i32(sa),
-                                           int(bool(keep_all)), hs))
+    _check(_L.da4ml_cmvm_solve_sweep_batch_seeded(n, kp, _ip(n_in), _ip(n_out), qp, lp, int(adder_size), int(carry_size), m, m0, m1, i32(hdc), i32(ddc), i32(sa), sd,
+                                                  int(bool(keep_all)), hs))  # fmt: skip
     return [SweepResult(_vp(h), k, [dict(s) for s in sets], None if q is None else [tuple(map(float, r)) for r in q], None if l is None else [float(v) for v in l],
                         int(adder_size), int(carry_size)) for h, k, q, l in zip(hs, ks, qs, ls)]
 
@@ -534,12 +580,43 @@ def solve_sweep(kernel, option_sets, qintervals=None, latencies=None, adder_size
     """Solve one matrix under every option set of ``option_sets`` in one GPU pass.
 
     Each option set is a dict of ``solve`` keywords (``method0, method1, hard_dc, decompose_dc,
-    search_all_decompose_dc``; missing keys take ``solve``'s defaults).  The intervals, latencies and the cost model
+    search_all_decompose_dc, seed``; missing keys take ``solve``'s defaults).  Sets that differ only in ``seed`` are
+    distinct candidates.  The intervals, latencies and the cost model
     (``adder_size``, ``carry_size``) are shared by all sets: costs under different cost models are not comparable.
     Op tables come back for the winners and the front, or for every candidate with ``keep_all``.  The batch of one
     matrix of ``solve_sweep_batch``."""
     return solve_sweep_batch([kernel], option_sets, None if qintervals is None else [qintervals], None if latencies is None else [latencies], adder_size, carry_size,
                              keep_all)[0]
+
+
+_SWEEP_CALL_KEYS = ('qintervals', 'latencies', 'adder_size', 'carry_size')  # solve() keywords that are arguments of a sweep
+
+
+def solve_best_of_raw(kernel, n_seeds=16, solver=None, **solve_kwargs) -> tuple[RawPipeline, int]:
+    """``solve_best_of`` as a ``RawPipeline``: ``(result, seed)``."""
+    if isinstance(n_seeds, bool) or not isinstance(n_seeds, (int, np.integer)) or n_seeds < 1:
+        raise ValueError(f'n_seeds must be a positive integer, got {n_seeds!r}')
+    if 'seed' in solve_kwargs:
+        raise TypeError('solve_best_of tries the seeds 0 .. n_seeds - 1 itself: it takes no seed keyword')
+    call = {k: solve_kwargs.pop(k) for k in _SWEEP_CALL_KEYS if k in solve_kwargs}
+    sets = [{**solve_kwargs, 'seed': s} for s in range(int(n_seeds))]
+    sw = (solve_sweep if solver is None else solver)(kernel, sets, **call)
+    winners = np.asarray(sw.winners, np.int64)
+    s = int(np.argmin(np.asarray(sw.candidates['cost'], np.float32)[winners]))  # (the first minimum: ties go to the lowest seed)
+    return sw.raw(int(winners[s])), s
+
+
+def solve_best_of(kernel, n_seeds=16, types_module=None, solver=None, **solve_kwargs):
+    """Best of ``n_seeds`` tie-break orders: ``solve(kernel, **solve_kwargs, seed=s)`` for ``s = 0 .. n_seeds - 1`` in one
+    GPU pass (a ``solve_sweep`` of one option set per seed), and the cheapest result.  Returns ``(Pipeline, seed)``.
+
+    Cost is ``SweepResult``'s float32 ``cost``; of equal costs the lowest seed wins, so the result is never costlier
+    than ``solve(kernel, **solve_kwargs)`` (seed 0) and is that result when no seed does better.  The returned design is
+    bit for bit what ``solve(kernel, **solve_kwargs, seed=seed)`` returns.  Every seed's greedy run is a valid run of the
+    same algorithm; a seed's graph is about as likely to be worse than seed 0's as better, and the gain is in keeping the
+    cheapest.  ``solver(kernel, option_sets, **kw)`` stands in for ``solve_sweep`` (same keywords and result)."""
+    raw, seed = solve_best_of_raw(kernel, n_seeds, solver, **solve_kwargs)
+    return raw.to_pipeline(types_module), seed
 
 
 NetworkPoint = namedtuple('NetworkPoint', ['cost', 'latency', 'choice'])
@@ -632,7 +709,8 @@ class ChainFront(NetworkFront):
     def reference_calls(self, p: int) -> list[dict]:
         """Per layer, the keywords of the ``solve(kernels[k], **kw)`` call that returns layer ``k``'s design in point
         ``p``: the candidate's options, the layer's ``qintervals`` and its input ``latencies`` as Python floats (for
-        ``k > 0``, the output latencies of the point's design of layer ``k - 1``)."""
+        ``k > 0``, the output latencies of the point's design of layer ``k - 1``).  A candidate of a seeded option set
+        carries its ``seed``, as ``SweepResult.reference_call`` does."""
         return copy.deepcopy(self._calls[p])
 
 
@@ -799,6 +877,7 @@ def cost_add(q0, q1, shift: int, sub: bool, adder_size: int, carry_size: int):
 
 __all__ = [
     'solve', 'solve_batch', 'solve_raw', 'solve_batch_raw', 'solve_batch_device_raw', 'solve_single_raw', 'solve_sweep', 'solve_sweep_batch', 'SweepResult', 'sweep_front',
+    'solve_best_of', 'solve_best_of_raw', 'tb_mask',
     'network_front', 'NetworkFront', 'NetworkPoint', 'chain_front', 'ChainFront', 'csd_decompose', 'int_arr_to_csd',
     'kernel_decompose', 'get_lsb_loc', 'iceil_log2', 'cost_add', 'dais_interp_run', 'device_info', 'plan', 'set_stream', 'set_group_size', 'set_accounting',
 ]  # fmt: skip

@@ -4,11 +4,13 @@
 GPU-side additions for many independent matrices, ``solve_sweep`` for one matrix under many option sets,
 ``solve_sweep_batch`` for many matrices under many option sets, ``network_front`` for the cheapest per-layer choice of a
 chain of layers under a latency budget, and ``chain_front`` for the same with each layer solved under the output latencies
-of the design before it (the designs and latencies a traced model gets)."""
+of the design before it (the designs and latencies a traced model gets).  ``solve``'s ``seed`` keyword picks the
+tie-break order of the greedy pair selection (0 = the reference's), and ``solve_best_of`` keeps the cheapest of many seeds."""
 
 from typing import TypedDict
 
-from .._binary import ChainFront, NetworkFront, SweepResult, chain_front, kernel_decompose, network_front, solve, solve_batch, solve_sweep, solve_sweep_batch
+from .._binary import (ChainFront, NetworkFront, SweepResult, chain_front, kernel_decompose, network_front, solve, solve_batch, solve_best_of, solve_sweep,
+                       solve_sweep_batch)  # fmt: skip
 from ..batching import CmvmCall, SolveBatcher, solve_calls
 from ..types import CombLogic, Op, Pipeline, QInterval
 
@@ -24,9 +26,10 @@ solver_options_t = TypedDict(
         'adder_size': int,
         'carry_size': int,
         'search_all_decompose_dc': bool,
+        'seed': int,
         'offload_fn': object,
     },
     total=False,
 )
 
-__all__ = ['solve', 'solve_batch', 'solve_sweep', 'solve_sweep_batch', 'SweepResult', 'network_front', 'NetworkFront', 'chain_front', 'ChainFront', 'solve_calls', 'CmvmCall', 'SolveBatcher', 'kernel_decompose', 'QInterval', 'Op', 'CombLogic', 'Pipeline', 'solver_options_t']
+__all__ = ['solve', 'solve_batch', 'solve_best_of', 'solve_sweep', 'solve_sweep_batch', 'SweepResult', 'network_front', 'NetworkFront', 'chain_front', 'ChainFront', 'solve_calls', 'CmvmCall', 'SolveBatcher', 'kernel_decompose', 'QInterval', 'Op', 'CombLogic', 'Pipeline', 'solver_options_t']

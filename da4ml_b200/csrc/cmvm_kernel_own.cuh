@@ -54,6 +54,7 @@ __device__ void solve_problem_own(const ProblemDesc &p, const Ctx &cx, const Own
 
     if (tid == 0) {
         b.seg_len = 0;
+        b.tb_mask = p.tb_mask;
         {
             // hot logs for the first expressions this CTA owns: its inputs and the earliest new expressions, the dense
             // rows that are rewritten again and again (not when the pool is too small to give each a few pages)
@@ -173,7 +174,7 @@ __device__ void solve_problem_own(const ProblemDesc &p, const Ctx &cx, const Own
             status = ST_EXPR_OVERFLOW;
             break;
         }
-        const uint64_t key = ((uint64_t)ch.khi << 32) | ch.klo;
+        const uint64_t key = ((uint64_t)ch.khi << 32) | ch.klo; // (collect_best has undone the tie-break mask)
         const uint32_t c0 = key_id0(key), c1 = key_id1(key);
         const int shift = key_shift(key), sub = key_sub(key);
         const uint32_t newid = (uint32_t)(n_in + t);

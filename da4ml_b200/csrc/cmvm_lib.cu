@@ -377,19 +377,42 @@ int da4ml_cmvm_solve_batch_device(
     });
 }
 
+int da4ml_cmvm_solve_seeded(
+    const float *kernel, int64_t n_in, int64_t n_out, const char *method0, const char *method1, int hard_dc, int decompose_dc,
+    const float *qintervals, const float *latencies, int adder_size, int carry_size, int search_all, uint64_t seed, da4ml_pipeline_t **out
+) {
+    return guarded([&] {
+        if (!kernel || !out || !method0 || !method1)
+            throw ApiError(DA4ML_E_INVALID, "invalid argument");
+        const float *ks[1] = {kernel};
+        const float *qs[1] = {qintervals};
+        const float *ls[1] = {latencies};
+        SolveOptions o{method0, method1, hard_dc, decompose_dc, search_all != 0};
+        o.seed = seed;
+        std::vector<std::unique_ptr<PipelineImpl>> res;
+        solve_many(1, ks, &n_in, &n_out, {o}, qs, ls, adder_size, carry_size, res);
+        *out = new da4ml_pipeline();
+        (*out)->impl = std::move(res[0]);
+    });
+}
+
 int da4ml_cmvm_solve(
     const float *kernel, int64_t n_in, int64_t n_out, const char *method0, const char *method1, int hard_dc, int decompose_dc,
     const float *qintervals, const float *latencies, int adder_size, int carry_size, int search_all, da4ml_pipeline_t **out
 ) {
-    const float *ks[1] = {kernel};
-    const float *qs[1] = {qintervals};
-    const float *ls[1] = {latencies};
-    return da4ml_cmvm_solve_batch(1, ks, &n_in, &n_out, method0, method1, hard_dc, decompose_dc, qs, ls, adder_size, carry_size, search_all, out);
+    return da4ml_cmvm_solve_seeded(kernel, n_in, n_out, method0, method1, hard_dc, decompose_dc, qintervals, latencies, adder_size, carry_size, search_all, 0, out);
 }
 
 int da4ml_cmvm_solve_single(
     const float *kernel, int64_t n_in, int64_t n_out, const char *method, const float *qintervals, const float *latencies,
     int adder_size, int carry_size, int32_t *trace, int64_t trace_cap, da4ml_pipeline_t **out
+) {
+    return da4ml_cmvm_solve_single_seeded(kernel, n_in, n_out, method, qintervals, latencies, adder_size, carry_size, trace, trace_cap, 0, out);
+}
+
+int da4ml_cmvm_solve_single_seeded(
+    const float *kernel, int64_t n_in, int64_t n_out, const char *method, const float *qintervals, const float *latencies,
+    int adder_size, int carry_size, int32_t *trace, int64_t trace_cap, uint64_t seed, da4ml_pipeline_t **out
 ) {
     return guarded([&] {
         if (!kernel || n_in <= 0 || n_out <= 0 || !method || !out)
@@ -408,6 +431,7 @@ int da4ml_cmvm_solve_single(
         j.method = parse_method(method);
         j.adder_size = adder_size;
         j.carry_size = carry_size;
+        j.seed = seed;
         j.d_kernel = (const float *)kbuf.p;
         j.qint.resize(3 * (size_t)n_in);
         j.lat.resize(n_in);
@@ -441,6 +465,15 @@ int da4ml_cmvm_solve_sweep_batch(
     const float *const *latencies, int adder_size, int carry_size, int64_t n_sets, const char *const *method0, const char *const *method1,
     const int32_t *hard_dc, const int32_t *decompose_dc, const int32_t *search_all, int keep_all, da4ml_sweep_t **out
 ) {
+    return da4ml_cmvm_solve_sweep_batch_seeded(n_problems, kernels, n_in, n_out, qintervals, latencies, adder_size, carry_size, n_sets, method0, method1, hard_dc,
+                                               decompose_dc, search_all, nullptr, keep_all, out);
+}
+
+int da4ml_cmvm_solve_sweep_batch_seeded(
+    int64_t n_problems, const float *const *kernels, const int64_t *n_in, const int64_t *n_out, const float *const *qintervals,
+    const float *const *latencies, int adder_size, int carry_size, int64_t n_sets, const char *const *method0, const char *const *method1,
+    const int32_t *hard_dc, const int32_t *decompose_dc, const int32_t *search_all, const uint64_t *seed, int keep_all, da4ml_sweep_t **out
+) {
     return guarded([&] {
         if (n_problems <= 0)
             throw ApiError(DA4ML_E_INVALID, "solve_sweep: n_problems must be positive (got " + std::to_string(n_problems) + ")");
@@ -461,6 +494,7 @@ int da4ml_cmvm_solve_sweep_batch(
             if (!method0[s] || !method1[s])
                 throw ApiError(DA4ML_E_INVALID, "solve_sweep: a method of option set " + std::to_string(s) + " is null");
             sets[s] = SolveOptions{method0[s], method1[s], hard_dc[s], decompose_dc[s], search_all[s] != 0};
+            sets[s].seed = seed ? seed[s] : 0;
             parse_method(sets[s].method0); // "Unknown method: ..." before any device call
             if (sets[s].method1 != "auto")
                 parse_method(sets[s].method1);

@@ -322,6 +322,19 @@ DA_HD uint32_t key_id0(uint64_t k) { return (uint32_t)(k >> 8) & 0x0fffffffu; }
 DA_HD int key_sub(uint64_t k) { return (int)(k >> 7) & 1; }
 DA_HD int key_shift(uint64_t k) { return (int)(k & 127) - 64; }
 
+// Seeded tie-break (this project's extension; the reference has only seed 0).  Among entries of equal score the greedy
+// selection takes the largest key ^ tb_mask(seed).  The mask covers the id0, sub and shift bits of pack_key and never
+// id1, so the newest expression still wins ties; tb_mask(0) = 0 is the reference's order.
+DA_HD uint64_t tb_mask(uint64_t seed) {
+    if (seed == 0)
+        return 0;
+    uint64_t x = seed + 0x9E3779B97F4A7C15ull; // splitmix64
+    x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
+    x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
+    x ^= x >> 31;
+    return x & ((1ull << 36) - 1);
+}
+
 // number of non-zero CSD digits of |x| (equals the digit count of bit_decompose.cc:22-42, which is
 // the non-adjacent form; equivalence is checked exhaustively in tests/test_numerics.py)
 DA_HD int csd_weight(int32_t x) {

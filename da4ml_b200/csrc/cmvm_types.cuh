@@ -53,6 +53,7 @@ struct ProblemDesc {
     int n_in, n_out;
     int method;
     int adder_size, carry_size;
+    unsigned long long tb_mask; // tie-break order of the greedy selection: tb_mask(seed) of cmvm_num.cuh, 0 = the reference's
     const float *kernel; // [n_in, n_out] row-major, device
     const float *qint;   // [n_in, 3]
     const float *lat;    // [n_in]

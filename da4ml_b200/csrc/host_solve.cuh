@@ -26,6 +26,7 @@ struct SolveOptions {
     std::string method0 = "wmc", method1 = "auto";
     int hard_dc = -1, decompose_dc = -2;
     bool search_all = true;
+    uint64_t seed = 0; // tie-break order of the greedy selection of both stages of every try (tb_mask, cmvm_num.cuh)
 };
 
 // A sweep's report on one candidate, i.e. one decompose_dc try of one option set (api.cc:190-201): the design that
@@ -70,6 +71,7 @@ struct Candidate {
     int hard_dc = -1;
     int decompose_dc = -2; // current value (after the api.cc:74-80 clamp)
     int adder_size = -1, carry_size = -1;
+    uint64_t seed = 0;
     float latency_allowed = std::numeric_limits<float>::infinity();
     // state
     int phase = 0; // 0: needs stage 0, 1: needs stage 1, 2: done
@@ -233,7 +235,7 @@ static void solve_many(
         }
     }
     // ---- candidates (api.cc:176-201).  Each (problem, set, try) is an entry; tries that start _solve in the same state
-    // (methods after api.cc:41-51, hard_dc, decompose_dc after the api.cc:74-80 clamp) are one candidate, solved once.
+    // (methods after api.cc:41-51, hard_dc, decompose_dc after the api.cc:74-80 clamp, seed) are one candidate, solved once.
     struct Entry {
         int problem, set, hard_dc, dc_start, cand;
     };
@@ -247,7 +249,7 @@ static void solve_many(
         bool latencies_small = true;
         for (float v : P.lat)
             latencies_small = latencies_small && std::isfinite(v) && std::fabs(v) < 1e6f;
-        std::map<std::tuple<std::string, std::string, int, int>, int> seen;
+        std::map<std::tuple<std::string, std::string, int, int, uint64_t>, int> seen;
         for (int si = 0; si < n_sets; ++si) {
             const SolveOptions &o = sets[si];
             std::vector<std::pair<int, int>> tries; // (hard_dc passed to _solve, decompose_dc passed to _solve)
@@ -267,6 +269,7 @@ static void solve_many(
                 c.hard_dc = tr.first;
                 c.adder_size = adder_size;
                 c.carry_size = carry_size;
+                c.seed = o.seed;
                 // api.cc:41-51
                 if (c.method1 == "auto")
                     c.method1 = (c.hard_dc >= 6 || ends_with(c.method0, "dc")) ? c.method0 : c.method0 + "-dc";
@@ -275,7 +278,7 @@ static void solve_many(
                 // api.cc:74-80
                 int log2_n = (int)std::ceil(std::log2((float)P.n_in));
                 c.decompose_dc = tr.second == -2 ? std::min(c.hard_dc, log2_n) : std::min({c.hard_dc, tr.second, log2_n});
-                const auto key = std::make_tuple(c.method0, c.method1, c.hard_dc, c.decompose_dc);
+                const auto key = std::make_tuple(c.method0, c.method1, c.hard_dc, c.decompose_dc, c.seed);
                 const auto it = seen.find(key);
                 if (it != seen.end()) {
                     entries.push_back(Entry{(int)pi, si, tr.first, tr.second, it->second});
@@ -416,6 +419,7 @@ static void solve_many(
                 j.method = parse_method(c.method0);
                 j.adder_size = c.adder_size;
                 j.carry_size = c.carry_size;
+                j.seed = c.seed;
                 j.d_kernel = c.d_m0;
                 j.qint = P.qint;
                 j.lat = P.lat;
@@ -428,6 +432,7 @@ static void solve_many(
                 j.method = parse_method(c.method1);
                 j.adder_size = c.adder_size;
                 j.carry_size = c.carry_size;
+                j.seed = c.seed;
                 j.d_kernel = c.d_m1;
                 j.cost_init = c.job0.res.cost_sum; // the float cost keeps accumulating across the two stages (api.cc:222-227)
                 // api.cc:100-115: stage-1 inputs are the RAW op qint/latency of the stage-0 outputs
@@ -471,6 +476,7 @@ static void solve_many(
                 auto put = [&](const void *p, size_t n) { k.append((const char *)p, n); };
                 const int head[6] = {c.problem, j.n_in, j.n_out, j.method, j.adder_size, j.carry_size};
                 put(head, sizeof(head));
+                put(&j.seed, sizeof(j.seed)); // (jobs that differ only in seed are different jobs)
                 put(&j.cost_init, sizeof(float));
                 put(j.qint.data(), sizeof(float) * j.qint.size());
                 put(j.lat.data(), sizeof(float) * j.lat.size());

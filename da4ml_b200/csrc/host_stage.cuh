@@ -32,6 +32,7 @@ struct StageResult {
 
 struct StageJob {
     int n_in = 0, n_out = 0, method = M_WMC, adder_size = -1, carry_size = -1;
+    uint64_t seed = 0;               // tie-break order of the greedy selection (tb_mask, cmvm_num.cuh); 0 = the reference's
     const float *d_kernel = nullptr; // device, [n_in][n_out]
     std::vector<float> qint, lat;    // host
     float cost_init = 0.0f; // float cost accumulated by the earlier stage(s) of the same candidate
@@ -174,6 +175,7 @@ static void run_stage_jobs(std::vector<StageJob *> &jobs, Timing &tm, bool want_
             d.method = j.method;
             d.adder_size = j.adder_size;
             d.carry_size = j.carry_size;
+            d.tb_mask = tb_mask(j.seed);
             d.kernel = j.d_kernel;
             d.qint = (const float *)(ja + off[i].qint);
             d.lat = (const float *)(ja + off[i].lat);

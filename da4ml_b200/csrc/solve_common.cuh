@@ -112,7 +112,7 @@ struct BlockCtx {
     Best warp_best[32];
     int warp_sum[32];
     int warp_st[32];
-    Best chosen;       // pair selected for the current step (score==0 -> none)
+    Best chosen;       // pair selected for the current step (score==0 -> none), key unmasked (see tb_mask below)
     // This CTA's histogram segment is a pool of `pages` pages of 2^chunk_log entries.  The common log fills it from page 0
     // upwards, [0, seg_len); the hot logs take single pages from its top downwards, [hot_top, pages), and give them back
     // to a free stack.  A hot log holds the entries whose passive partner is one of the first hot_n expressions this CTA
@@ -146,6 +146,10 @@ struct BlockCtx {
     int r_step;        // digit pairs enumerated in the current step
     int rescan_step;   // histogram entries re-read in the current step
     unsigned long long xw[3]; // a group of one CTA: the payload words of its exchange
+    // The problem's tie-break mask (ProblemDesc::tb_mask).  Histogram entries, page caches, Bests and the exchange carry
+    // pack_key ^ tb_mask, so that every comparison of (score, key) applies the seeded order as it stands; whoever reads
+    // id0, sub or shift out of a key XORs the mask back first (id1 is never masked).
+    unsigned long long tb_mask;
 };
 
 struct Ctx {
@@ -332,7 +336,7 @@ emit_entry(const ProblemDesc &p, const Ctx &cx, uint32_t lo, uint32_t hi, int sh
     uint32_t score;
     if (!pair_score(p.method, count, q0, l0, q1, l1, score))
         return; // NaN score: can never be selected
-    const uint64_t key = pack_key(lo, hi, shift, sub);
+    const uint64_t key = pack_key(lo, hi, shift, sub) ^ cx.b->tb_mask;
     int pos = -1;
     if (hot >= 0) { // the passive partner's own log; when its pages are full the entry goes to the common log like any other
         const int q = smem_add(&cx.b->hot_len[hot], 1);

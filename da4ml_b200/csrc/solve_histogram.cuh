@@ -6,11 +6,12 @@
 namespace da {
 
 // ---- lazy histogram -------------------------------------------------------------------------------
-__device__ __forceinline__ bool entry_live(const FEnt &e, const uint32_t *mod, uint32_t c0, uint32_t c1, bool purge) {
+// (`m0` = key_id0 of the tie-break mask: the entry's key is stored masked)
+__device__ __forceinline__ bool entry_live(const FEnt &e, const uint32_t *mod, uint32_t c0, uint32_t c1, bool purge, uint32_t m0) {
     if (e.y == DA_DEAD)
         return false;
     const uint64_t key = ((uint64_t)e.w << 32) | e.z;
-    const uint32_t a = key_id0(key), c = key_id1(key);
+    const uint32_t a = key_id0(key) ^ m0, c = key_id1(key);
     if (purge && (a == c0 || a == c1 || c == c0 || c == c1))
         return false;
     const uint32_t ma = __ldcg(&mod[a]), mc = __ldcg(&mod[c]);
@@ -23,6 +24,7 @@ __device__ __forceinline__ bool entry_live(const FEnt &e, const uint32_t *mod, u
 __device__ __forceinline__ int rescan_range(const Ctx &cx, int lo, int hi, uint32_t c0, uint32_t c1, bool purge, uint32_t thresh, Best &out) {
     const int lane = threadIdx.x & 31;
     const uint32_t *mod = cx.ws.mod_step;
+    const uint32_t m0 = key_id0(cx.b->tb_mask);
     Best best{0u, 0u, 0u};
     int live = 0;
     constexpr int U = 8;
@@ -41,7 +43,7 @@ __device__ __forceinline__ int rescan_range(const Ctx &cx, int lo, int hi, uint3
             ma[u] = mc[u] = 0u;
             if (e[u].y != DA_DEAD) {
                 const uint64_t key = ((uint64_t)e[u].w << 32) | e[u].z;
-                ma[u] = __ldcg(&mod[key_id0(key)]);
+                ma[u] = __ldcg(&mod[key_id0(key) ^ m0]);
                 mc[u] = __ldcg(&mod[key_id1(key)]);
             }
         }
@@ -50,7 +52,7 @@ __device__ __forceinline__ int rescan_range(const Ctx &cx, int lo, int hi, uint3
             if (e[u].y == DA_DEAD)
                 continue;
             const uint64_t key = ((uint64_t)e[u].w << 32) | e[u].z;
-            const uint32_t a = key_id0(key), c = key_id1(key);
+            const uint32_t a = key_id0(key) ^ m0, c = key_id1(key);
             const bool ok = !(purge && (a == c0 || a == c1 || c == c0 || c == c1)) && e[u].y >= ma[u] && e[u].y >= mc[u];
             if (ok) {
                 ++live;
@@ -92,7 +94,7 @@ __device__ void refresh_chunks(const Ctx &cx, const Team &tm, int seg_len, uint3
         bool d = all || cx.cb_dirty[c];
         if (!d && purge && cx.cb_score[c] != 0u) {
             const uint64_t key = ((uint64_t)cx.cb_khi[c] << 32) | cx.cb_klo[c];
-            const uint32_t a = key_id0(key), e = key_id1(key);
+            const uint32_t a = key_id0(key ^ b.tb_mask), e = key_id1(key);
             d = (a == c0 || a == c1 || e == c0 || e == c1);
         }
         if (d)
@@ -286,6 +288,7 @@ __device__ __noinline__ void compact_segment(const Ctx &cx, uint32_t c0, uint32_
     const int tid = threadIdx.x, nt = blockDim.x, lane = tid & 31;
     BlockCtx &b = *cx.b;
     const int len = b.seg_len;
+    const uint32_t m0 = key_id0(b.tb_mask);
     constexpr int K = 8;
     if (tid == 0)
         b.cmp_out = 0;
@@ -299,7 +302,7 @@ __device__ __noinline__ void compact_segment(const Ctx &cx, uint32_t c0, uint32_
             live[k] = false;
             if (i < len) {
                 e[k] = __ldcg(&cx.seg[i]);
-                live[k] = entry_live(e[k], cx.ws.mod_step, c0, c1, purge);
+                live[k] = entry_live(e[k], cx.ws.mod_step, c0, c1, purge, m0);
             }
         }
         __syncthreads(); // every read of this tile is complete
@@ -419,7 +422,7 @@ __device__ int collect_best(const Ctx &cx, int pw) {
             st = max(st & 0xff, o & 0xff) | ((st | o) & 0x100);
         }
         if (lane == 0) {
-            b.chosen = v;
+            b.chosen = Best{v.score, v.khi ^ (uint32_t)(b.tb_mask >> 32), v.klo ^ (uint32_t)b.tb_mask}; // (the key as pack_key formed it)
             b.scratch_i[0] = live;
             b.scratch_i[1] = st & 0xff;
             b.scratch_i[3] = (st >> 8) & 1;

@@ -76,6 +76,18 @@ int da4ml_cmvm_solve(
     int carry_size, int search_all_decompose_dc, da4ml_pipeline_t **out
 );
 
+/* Seeded tie-breaks (this library's extension; the reference has seed 0 only).  Among histogram entries of equal selector
+ * score the greedy selection takes the one whose (packed key ^ tb_mask(seed)) is largest, where the packed key is
+ * (id1 << 36 | id0 << 8 | sub << 7 | shift + 64) and tb_mask(0) = 0, tb_mask(s) = splitmix64(s) & (2^36 - 1): id1 is never
+ * masked.  Seed 0 is the reference's rule exactly, and another seed is an equally valid greedy run with a different graph.
+ * The seed applies to the greedy loop of both stages of every decompose_dc try; the decomposition, the latency retries,
+ * the adder trees and the argmin over the tries are unchanged.  da4ml_cmvm_solve is the case seed = 0. */
+int da4ml_cmvm_solve_seeded(
+    const float *kernel, int64_t n_in, int64_t n_out, const char *method0, const char *method1,
+    int hard_dc, int decompose_dc, const float *qintervals, const float *latencies, int adder_size,
+    int carry_size, int search_all_decompose_dc, uint64_t seed, da4ml_pipeline_t **out
+);
+
 /* Batched form of da4ml_cmvm_solve: n independent problems solved concurrently on one GPU (the
  * reference has no batch API; its caller loops, trace/fixed_variable_array.py:368-371).  Per-problem
  * arrays of pointers; qintervals[i] / latencies[i] (or the arrays themselves) may be NULL.        */
@@ -101,6 +113,13 @@ int da4ml_cmvm_solve_batch_device(
 int da4ml_cmvm_solve_single(
     const float *kernel, int64_t n_in, int64_t n_out, const char *method, const float *qintervals,
     const float *latencies, int adder_size, int carry_size, int32_t *trace, int64_t trace_cap,
+    da4ml_pipeline_t **out
+);
+/* The same under a tie-break seed (see da4ml_cmvm_solve_seeded); the trace reports the pairs the seeded run chose.
+ * da4ml_cmvm_solve_single is the case seed = 0. */
+int da4ml_cmvm_solve_single_seeded(
+    const float *kernel, int64_t n_in, int64_t n_out, const char *method, const float *qintervals,
+    const float *latencies, int adder_size, int carry_size, int32_t *trace, int64_t trace_cap, uint64_t seed,
     da4ml_pipeline_t **out
 );
 
@@ -137,6 +156,16 @@ int da4ml_cmvm_solve_sweep_batch(
     const float *const *latencies, int adder_size, int carry_size, int64_t n_sets, const char *const *method0,
     const char *const *method1, const int32_t *hard_dc, const int32_t *decompose_dc, const int32_t *search_all, int keep_all,
     da4ml_sweep_t **out /* [n_problems] */
+);
+/* The same with a tie-break seed per option set (seed[s], see da4ml_cmvm_solve_seeded; NULL = all 0).  Sets that differ
+ * only in seed are distinct candidates; a candidate's seed is its set's.  Candidate c is the result of
+ * da4ml_cmvm_solve_seeded(kernel, method0, method1, H, d, search_all_decompose_dc = 0, ..., seed[set]) bit for bit.
+ * da4ml_cmvm_solve_sweep_batch is the case seed = NULL. */
+int da4ml_cmvm_solve_sweep_batch_seeded(
+    int64_t n_problems, const float *const *kernels, const int64_t *n_in, const int64_t *n_out, const float *const *qintervals,
+    const float *const *latencies, int adder_size, int carry_size, int64_t n_sets, const char *const *method0,
+    const char *const *method1, const int32_t *hard_dc, const int32_t *decompose_dc, const int32_t *search_all,
+    const uint64_t *seed /* [n_sets] or NULL */, int keep_all, da4ml_sweep_t **out /* [n_problems] */
 );
 /* counts: {n_sets, n_candidates, n_kept (candidates with op tables), n_solved (distinct candidates solved)} */
 int da4ml_sweep_counts(const da4ml_sweep_t *s, int64_t out[4]);
