@@ -85,6 +85,9 @@ _L.da4ml_dais_program_free.restype = None
 _L.da4ml_cmvm_get_lsb_loc.argtypes = [C.c_float]
 _L.da4ml_cmvm_iceil_log2.argtypes = [C.c_float]
 _L.da4ml_cmvm_cost_add.argtypes = [_f32p, _f32p, C.c_int64, C.c_int, C.c_int, C.c_int, _f32p]
+_f64p = C.POINTER(C.c_double)
+_L.da4ml_pipeline_price.argtypes = [C.c_int64, _i64p, _i64p, _i64p, _i64p, _i64p, _i64p, _i64p, _f32p, _f64p, _f64p, C.c_int64, C.c_int, _i32p, _i64p, _i64p, _f64p,
+                                    _f64p, _f64p, _f64p]  # fmt: skip
 
 EXPORTED_SYMBOLS = [
     'da4ml_cmvm_last_error', 'da4ml_cmvm_device_info', 'da4ml_cmvm_set_stream', 'da4ml_cmvm_set_group_size',
@@ -97,7 +100,7 @@ EXPORTED_SYMBOLS = [
     'da4ml_dais_program_load', 'da4ml_dais_program_info', 'da4ml_dais_program_run', 'da4ml_dais_program_run_stream',
     'da4ml_dais_program_free', 'da4ml_dais_program_profile', 'da4ml_dais_program_dump', 'da4ml_cmvm_solve_sweep', 'da4ml_cmvm_solve_sweep_batch', 'da4ml_sweep_counts',
     'da4ml_sweep_profile', 'da4ml_sweep_summary', 'da4ml_sweep_pipeline', 'da4ml_sweep_free', 'da4ml_sweep_front',
-    'da4ml_cmvm_solve_seeded', 'da4ml_cmvm_solve_single_seeded', 'da4ml_cmvm_solve_sweep_batch_seeded',
+    'da4ml_cmvm_solve_seeded', 'da4ml_cmvm_solve_single_seeded', 'da4ml_cmvm_solve_sweep_batch_seeded', 'da4ml_pipeline_price',
 ]  # fmt: skip
 
 COUNTER_NAMES = ['status', 'n_ops', 'T', 'sum_F', 'sum_R', 'F0', 'R0', 'D_final', 'F_max', 'compactions', 'D0', 'n_bits', 'group_ctas',
@@ -517,6 +520,18 @@ class SweepResult:
             call['seed'] = int(s['seed'])
         return call
 
+    def pipelined(self, latency_cutoff, retiming: bool = True, pricer=None) -> 'PipelinePrice':
+        """``price_pipelined`` of every candidate whose op tables were kept, under the sweep's own input latencies, in one
+        call.  The arrays are aligned with ``candidates`` (``[len(self), n_cutoffs]``); a candidate that was not kept has
+        status -1, ``stages`` / ``reg_bits`` -1 and NaN latencies.  Only the winners and the front are kept unless the
+        sweep ran with ``keep_all=True``, which is needed to price every candidate.  ``pricer`` stands in for
+        ``price_pipelined``."""
+        kept = np.flatnonzero(self.candidates['kept'])
+        lat = self._call['latencies']
+        pr = (price_pipelined if pricer is None else pricer)([self.raw(int(i)) for i in kept], latency_cutoff, latencies=None if lat is None else [lat] * kept.size,
+                                                             retiming=retiming)  # fmt: skip
+        return pr._scatter(kept, len(self))
+
 
 def _prefixed(tag, f, *args, **kw):
     try:
@@ -694,9 +709,22 @@ class ChainFront(NetworkFront):
 
     Only host arrays are held (each point's designs are ``RawPipeline`` copies), so a front pickles as it is."""
 
-    def __init__(self, cost, latency, choice, raws, calls, profile):
+    def __init__(self, cost, latency, choice, raws, calls, profile, latency_cutoff=0.0):
         super().__init__(cost, latency, choice)
         self._raws, self._calls, self.profile = raws, calls, profile
+        self.latency_cutoff = float(latency_cutoff)
+        c = self.latency_cutoff
+        # (to_pipeline's stage of the last output, + 1: the clock count of a chain whose network inputs arrive before c)
+        self.stages = (np.floor(np.asarray(latency, np.float64) / (c + 1e-9)).astype(np.int64) + 1) if c > 0 else np.ones(len(cost), np.int64)
+
+    def best_stages(self, n_stages) -> NetworkPoint:
+        """The cheapest point with at most ``n_stages`` register stages (the first of equal ones); ``ValueError`` when
+        every point needs more."""
+        ok = np.flatnonzero(self.stages <= int(n_stages))
+        if ok.size == 0:
+            raise ValueError(f'no design of the network fits in {n_stages} stages (the fastest needs {int(self.stages.min())})')
+        p = int(ok[np.argmin(self.cost[ok])])
+        return NetworkPoint(float(self.cost[p]), float(self.latency[p]), tuple(int(c) for c in self.choice[p]))
 
     def raw(self, p: int, k: int) -> RawPipeline:
         """Layer ``k``'s design in point ``p``."""
@@ -714,16 +742,23 @@ class ChainFront(NetworkFront):
         return copy.deepcopy(self._calls[p])
 
 
-def _chain_layer(points, state_of, sweeps, state_lats):
+def _chain_layer(points, state_of, sweeps, state_lats, traced=None):
     """Extend the points of the layers so far by the next layer and prune.  ``points`` is ``None`` at layer 0, else
     ``(cost, lat, choice, outs, raws, calls)``; ``state_of[p]`` is the index of point ``p``'s input-latency state in
     ``sweeps`` and ``state_lats`` (lists of Python floats); at layer 0 there is one state and ``state_of == [0]``.
     Parents are taken in order and each is extended by every ``front`` candidate of its state's sweep, in candidate
     order; cost is the float32 sum in layer order, latency the new design's ``latency_max``; then the ``sweep_front``
-    rule.  ``outs[p]`` are the output latencies of point ``p``'s last design."""
+    rule.  ``outs[p]`` are the output latencies of point ``p``'s last design.  ``traced[s, i]`` (pipelined chains):
+    ``(latency_max, output latencies)`` of front candidate ``i`` of state ``s`` as traced under the cutoff, which replace the
+    solver's; a front candidate without an entry is dropped."""
     fronts = [np.asarray(sw.front, np.int64) for sw in sweeps]
+    if traced is not None:
+        fronts = [np.asarray([i for i in f.tolist() if (s, i) in traced], np.int64) for s, f in enumerate(fronts)]
     f_cost = [np.asarray(sw.candidates['cost'], np.float32)[f] for sw, f in zip(sweeps, fronts)]
-    f_lat = [np.asarray(sw.candidates['latency_max'], np.float32)[f] for sw, f in zip(sweeps, fronts)]
+    if traced is None:
+        f_lat = [np.asarray(sw.candidates['latency_max'], np.float32)[f] for sw, f in zip(sweeps, fronts)]
+    else:
+        f_lat = [np.asarray([traced[s, i][0] for i in f.tolist()], np.float64) for s, f in enumerate(fronts)]
     par = np.concatenate([np.full(fronts[s].size, p, np.int64) for p, s in enumerate(state_of)])
     sidx = np.concatenate([np.full(fronts[s].size, s, np.int64) for s in state_of])
     cand = np.concatenate([fronts[s] for s in state_of])
@@ -739,7 +774,7 @@ def _chain_layer(points, state_of, sweeps, state_lats):
     for p, s, i in zip(par.tolist(), sidx.tolist(), cand.tolist()):
         if (s, i) not in designs:
             r = sweeps[s].raw(i)
-            designs[s, i] = (r, {**sweeps[s].reference_call(i), 'latencies': state_lats[s]}, _out_latencies(r))
+            designs[s, i] = (r, {**sweeps[s].reference_call(i), 'latencies': state_lats[s]}, _out_latencies(r) if traced is None else traced[s, i][1])
         r, call, o = designs[s, i]
         raws.append([r] if points is None else [*points[4][p], r])
         calls.append([call] if points is None else [*points[5][p], call])
@@ -747,7 +782,7 @@ def _chain_layer(points, state_of, sweeps, state_lats):
     return cost, lat, choice, outs, raws, calls
 
 
-def chain_front(kernels, option_sets, qintervals=None, latencies=None, adder_size=-1, carry_size=-1, solver=None) -> ChainFront:
+def chain_front(kernels, option_sets, qintervals=None, latencies=None, adder_size=-1, carry_size=-1, solver=None, latency_cutoff=0.0, pricer=None) -> ChainFront:
     """The cost / latency front of a chain of layers, each layer solved under the output latencies of the design chosen
     for the layer before it, as a traced model's matmuls are: every reported design is what
     ``solve(kernels[k], **front.reference_calls(p)[k])`` returns, and every reported cost and latency is the chain's own.
@@ -766,15 +801,25 @@ def chain_front(kernels, option_sets, qintervals=None, latencies=None, adder_siz
     design's ``latency_max``, which already contains the upstream latency.  The points are pruned after each layer with
     the ``sweep_front`` rule, and the result is sorted by ascending latency.
 
-    Latency model: latency is the solver's op latency.  Activations between layers add none, as ``relu`` and ``wrap`` in
-    the tracer keep their input's latency, and ``latency_cutoff > 0`` pipelining is not modelled.  The front is the front
-    of the chains explored: the solver is not monotone in its input latencies, so pruning partial chains on (cost,
-    ``latency_max``) is a heuristic and a pruned chain could have led to a better design.  What is reported is exact.
+    Latency model: with ``latency_cutoff = 0`` (the default) latency is the solver's op latency.  With ``latency_cutoff =
+    c > 0`` it is the latency the tracer gives the design under ``HWConfig(adder_size, carry_size, c)``: after each
+    layer's sweep every front candidate of every state is priced under that state's latencies (``price_pipelined``
+    without retiming, one call per layer); a point's latency is the traced ``latency_max``, its next state the traced
+    output latencies (what the traced model hands the next ``solve``), pruning uses (cost, traced latency), and a
+    candidate whose status is not ok (an adder slower than ``c``) is dropped (``profile['layers'][k]['dropped']``).
+    ``stages[p] = floor(latency / (c + 1e-9)) + 1`` is the clock count ``to_pipeline`` gives the chain when its network
+    inputs arrive before ``c``; ``retime_pipeline`` never accepts a split with more stages, so retiming never adds a
+    clock.  ``best_stages(n)`` is the cheapest point with at most ``n`` stages.  Register bits of a whole chain are not
+    reported: the activation ops between layers have widths of their own, so they are not the sum of the layers'.
+    Activations between layers add no latency, as ``relu`` and ``wrap`` in the tracer keep their input's latency.  The
+    front is the front of the chains explored: the solver is not monotone in its input latencies, so pruning partial
+    chains on (cost, latency) is a heuristic and a pruned chain could have led to a better design.  What is reported is
+    exact.
 
     Limits: a layer's states all run in one call, and their op tables stay on the device until that call ends; if they do
     not fit (``DA4ML_E_CAPACITY``), or any set fails on any state, the call raises that layer's error prefixed with
     ``layer k: `` and returns nothing.  Branching networks are not covered.  ``solver(kernels, option_sets, **kw)`` stands
-    in for ``solve_sweep_batch`` (same keywords and results)."""
+    in for ``solve_sweep_batch`` (same keywords and results), ``pricer`` for ``price_pipelined``."""
     ks = [_prefixed(f'layer {k}', _kernel_arg, W) for k, W in enumerate(kernels)]
     if not ks:
         raise ValueError('chain_front needs at least one layer')
@@ -787,28 +832,156 @@ def chain_front(kernels, option_sets, qintervals=None, latencies=None, adder_siz
     qs = [None if qintervals is None else _prefixed(f'layer {k}', _qint_arg, qintervals[k], W.shape[0]) for k, W in enumerate(ks)]
     qs = [None if q is None else [tuple(map(float, r)) for r in q] for q in qs]
     l0 = _prefixed('layer 0', _lat_arg, latencies, ks[0].shape[0])
-    states = [np.zeros(ks[0].shape[0], np.float32) if l0 is None else l0]
+    c = float(latency_cutoff)
+    if not (c >= 0 and np.isfinite(c)):
+        raise ValueError(f'latency_cutoff must be a non-negative number, got {latency_cutoff!r}')
+    dt = np.float64 if c > 0 else np.float32  # (traced latencies are the tracer's doubles)
+    states = [np.zeros(ks[0].shape[0], dt) if l0 is None else l0.astype(dt)]
     solver = solve_sweep_batch if solver is None else solver
+    pricer = price_pipelined if pricer is None else pricer
     prof = dict(launches=0, device_ms=0.0, jobs_run=0, jobs_total=0, layers=[])
     points, state_of = None, np.zeros(1, np.int64)
     for k, W in enumerate(ks):
         if k > 0:  # one state per distinct output-latency vector, in order of first use
             index = {}
-            state_of = np.asarray([index.setdefault(o.tobytes(), len(index)) for o in points[3]], np.int64)
-            states = [np.frombuffer(b, np.float32) for b in index]
+            state_of = np.asarray([index.setdefault(np.asarray(o, dt).tobytes(), len(index)) for o in points[3]], np.int64)
+            states = [np.frombuffer(b, dt) for b in index]
         n, lats = len(states), [[float(v) for v in s] for s in states]
         sweeps = _prefixed(f'layer {k}', solver, [W] * n, sets, qintervals=[qs[k]] * n, latencies=lats, adder_size=int(adder_size), carry_size=int(carry_size))
-        points = _chain_layer(points, state_of, sweeps, lats)
+        traced, priced = None, {}
+        if c > 0:  # every front candidate of every state, traced under its state's latencies: one pricing call
+            keys = [(s, int(i)) for s, sw in enumerate(sweeps) for i in np.asarray(sw.front, np.int64).tolist()]
+            pr = _prefixed(f'layer {k}', pricer, [sweeps[s].raw(i) for s, i in keys], c, latencies=[lats[s] for s, _ in keys], retiming=False)
+            traced = {key: (float(pr.latency_max[j, 0]), np.asarray(pr.out_latency(j, 0), np.float64)) for j, key in enumerate(keys) if int(pr.status[j, 0]) == 0}
+            priced = dict(dropped=len(keys) - len(traced), price_launches=int(pr.profile.get('launches', 0)), price_device_ms=float(pr.profile.get('device_ms', 0.0)))
+        points = _chain_layer(points, state_of, sweeps, lats, traced)
+        if len(points[0]) == 0:
+            raise ValueError(f'layer {k}: every front candidate has an adder slower than the latency cutoff {c}')
         p0 = sweeps[0].profile  # (the whole call's)
         layer = dict(states=n, candidates=sum(len(sw.candidates['cost']) for sw in sweeps), points=len(points[0]),
-                     **{key: p0[key] for key in ('launches', 'device_ms', 'jobs_run', 'jobs_total')})
+                     **{key: p0[key] for key in ('launches', 'device_ms', 'jobs_run', 'jobs_total')}, **priced)
         prof['layers'].append(layer)
         for key in ('launches', 'device_ms', 'jobs_run', 'jobs_total'):
             prof[key] += layer[key]
         del sweeps  # (the designs are copied out: free the handles before the next layer's call)
     cost, lat, choice, _, raws, calls = points
     order = np.argsort(lat, kind='stable')
-    return ChainFront(cost[order], lat[order], choice[order], [raws[p] for p in order], [calls[p] for p in order], prof)
+    return ChainFront(cost[order], lat[order], choice[order], [raws[p] for p in order], [calls[p] for p in order], prof, c)
+
+
+PRICE_STATUS = ['ok', 'adder slower than the cutoff', 'not supported']  # PipelinePrice.status codes 0, 1, 2
+
+
+class PipelinePrice:
+    """What ``price_pipelined`` returns: arrays ``[n_designs, n_cutoffs]`` -- ``status`` (int32: 0 ok, 1 an adder is
+    slower than the cutoff, the tracer's ``AssertionError``; 2 not supported, a constant intermediate value that
+    ``emit`` refuses too; names in ``PRICE_STATUS``), ``stages`` (the number of register stages of the split),
+    ``reg_bits`` (``Pipeline.reg_bits`` of the split), ``latency_max`` (the traced output latencies' maximum, float64)
+    and ``cutoff`` (the cutoff retiming settled on, or the cutoff itself without retiming), ``cutoffs`` (the cutoffs
+    asked for), and ``out_latency(d, j)``: design ``d``'s traced output latencies under cutoff ``j``.  A task that is not
+    ok has ``stages`` and ``reg_bits`` -1 and NaN latencies.  ``profile``: the call's device time and launches."""
+
+    def __init__(self, status, stages, reg_bits, latency_max, cutoff, cutoffs, out_lat, profile):
+        self.status, self.stages, self.reg_bits, self.latency_max, self.cutoff = status, stages, reg_bits, latency_max, cutoff
+        self.cutoffs, self._out_lat, self.profile = cutoffs, out_lat, profile
+
+    def __len__(self):
+        return len(self.status)
+
+    @property
+    def ok(self) -> np.ndarray:
+        return self.status == 0
+
+    def out_latency(self, d: int, j: int = 0) -> np.ndarray:
+        """Traced latency of every output of design ``d`` under cutoff ``j`` (float64; 0.0 for a dead column)."""
+        o = self._out_lat[int(d)]
+        if o is None:
+            raise ValueError(f'design {d} was not priced (its op tables were not kept)')
+        return o[int(j)].copy()
+
+    def _scatter(self, rows, n) -> 'PipelinePrice':
+        """The same answers at rows ``rows`` of ``n`` (the others: not priced)."""
+        m = len(self.cutoffs)
+
+        def put(a, fill):
+            out = np.full((n, m), fill, a.dtype)
+            out[rows] = a
+            return out
+
+        out_lat = [None] * n
+        for k, r in enumerate(np.asarray(rows, np.int64).tolist()):
+            out_lat[r] = self._out_lat[k]
+        return PipelinePrice(put(self.status, -1), put(self.stages, -1), put(self.reg_bits, -1), put(self.latency_max, np.nan), put(self.cutoff, np.nan),
+                             self.cutoffs, out_lat, self.profile)  # fmt: skip
+
+
+def _design_stages(design) -> list[dict]:
+    from ..emit import _stages_of
+
+    return _stages_of(design)
+
+
+def _price_args(designs, latency_cutoff, latencies) -> dict:
+    """The flat arrays of ``da4ml_pipeline_price`` for ``price_pipelined``'s arguments."""
+    if hasattr(designs, 'stages') or hasattr(designs, 'solutions') or isinstance(designs, dict):
+        designs = [designs]
+    designs = [_design_stages(d) for d in designs]
+    if not designs:
+        raise ValueError('price_pipelined needs at least one design')
+    cut = np.ascontiguousarray(np.atleast_1d(np.asarray(latency_cutoff, np.float64)).ravel())
+    if cut.size == 0:
+        raise ValueError('price_pipelined needs at least one latency cutoff')
+    stages = [st for d in designs for st in d]
+    meta = np.asarray([[st['shape'][0], st['shape'][1], len(st['ops_i']), st['carry_size'], st['adder_size']] for st in stages], np.int64).reshape(-1, 5)
+    cat = lambda key, w: np.ascontiguousarray(np.concatenate([np.asarray(st[key], np.int64).reshape(-1, w) for st in stages]).ravel())  # noqa: E731
+    ops_f = np.ascontiguousarray(np.concatenate([np.asarray(st['ops_f'], np.float32).reshape(-1, 5) for st in stages]).ravel())
+    lat = None
+    if latencies is not None:
+        if len(latencies) != len(designs):
+            raise ValueError(f'expected latencies for {len(designs)} designs, got {len(latencies)}')
+        parts = []
+        for d, l in zip(designs, latencies):
+            n_in = d[0]['shape'][0]
+            v = np.zeros(n_in) if l is None or len(l) == 0 else np.asarray(list(l), np.float64).ravel()
+            if v.size != n_in:
+                raise ValueError(f'expected {n_in} latencies, got {v.size}')
+            parts.append(v)
+        lat = np.ascontiguousarray(np.concatenate(parts) if parts else np.zeros(0))
+    return dict(designs=designs, cutoffs=cut, latencies=lat, n_stages=np.asarray([len(d) for d in designs], np.int64), meta=np.ascontiguousarray(meta.ravel()),
+                inp_shifts=cat('inp_shifts', 1), out_idxs=cat('out_idxs', 1), out_shifts=cat('out_shifts', 1), out_negs=cat('out_negs', 1), ops_i=cat('ops_i', 4),
+                ops_f=ops_f)  # fmt: skip
+
+
+def price_pipelined(designs, latency_cutoff, latencies=None, retiming: bool = True) -> PipelinePrice:
+    """Price designs as they will be pipelined, on the GPU: for every design and every cutoff ``c`` what the reference gets
+    by replaying the design through its tracer under ``HWConfig(adder_size, carry_size, c)`` with its inputs at
+    ``latencies``, gathering it with ``comb_trace`` and splitting it with ``to_pipeline(comb, c, retiming)``.
+
+    ``designs``: a sequence of ``RawPipeline``s, stage-dict lists or ``Pipeline`` containers (or one of them).
+    ``latency_cutoff``: a positive number or a sequence of them.  ``latencies``: ``None`` (zeros) or, per design, ``None``
+    or its input latencies.  With ``retiming`` the split is the one ``retime_pipeline`` keeps; its bisection re-traces
+    with every input at latency 0, as the reference re-traces a split.  Traced latencies are those of the first trace
+    (the given latencies and cutoff), as the next layer's tracer would see them.
+
+    A task that is not ``ok`` (an adder slower than the cutoff, a constant intermediate value) does not raise: it is
+    reported in ``status``, so one slow adder does not fail a sweep.  Argument errors raise ``ValueError`` before any
+    device call."""
+    pk = _price_args(designs, latency_cutoff, latencies)
+    designs, cut, lat = pk['designs'], pk['cutoffs'], pk['latencies']
+    n, m = len(designs), cut.size
+    n_out = [d[-1]['shape'][1] for d in designs]
+    st_ = np.zeros(n * m, np.int32)
+    stg, rb = np.zeros(n * m, np.int64), np.zeros(n * m, np.int64)
+    lm, co = np.zeros(n * m), np.zeros(n * m)
+    ol = np.zeros(sum(n_out) * m)
+    prof = np.zeros(2)
+    f64 = lambda a: a.ctypes.data_as(_f64p) if a is not None else None  # noqa: E731
+    _check(_L.da4ml_pipeline_price(n, *[_ip(pk[k]) for k in ('n_stages', 'meta', 'inp_shifts', 'out_idxs', 'out_shifts', 'out_negs', 'ops_i')], _fp(pk['ops_f']),
+                                   f64(lat), f64(cut), m, int(bool(retiming)), st_.ctypes.data_as(_i32p), _ip(stg), _ip(rb), f64(lm), f64(co), f64(ol), f64(prof)))  # fmt: skip
+    edges = np.concatenate([[0], np.cumsum(np.asarray(n_out, np.int64) * m)])
+    out_lat = [ol[edges[d] : edges[d + 1]].reshape(m, n_out[d]) for d in range(n)]
+    return PipelinePrice(st_.reshape(n, m), stg.reshape(n, m), rb.reshape(n, m), lm.reshape(n, m), co.reshape(n, m), cut, out_lat,
+                         dict(device_ms=float(prof[0]), launches=int(prof[1])))  # fmt: skip
 
 
 def csd_decompose(inp, center=True):
@@ -877,7 +1050,7 @@ def cost_add(q0, q1, shift: int, sub: bool, adder_size: int, carry_size: int):
 
 __all__ = [
     'solve', 'solve_batch', 'solve_raw', 'solve_batch_raw', 'solve_batch_device_raw', 'solve_single_raw', 'solve_sweep', 'solve_sweep_batch', 'SweepResult', 'sweep_front',
-    'solve_best_of', 'solve_best_of_raw', 'tb_mask',
+    'solve_best_of', 'solve_best_of_raw', 'tb_mask', 'price_pipelined', 'PipelinePrice', 'PRICE_STATUS',
     'network_front', 'NetworkFront', 'NetworkPoint', 'chain_front', 'ChainFront', 'csd_decompose', 'int_arr_to_csd',
     'kernel_decompose', 'get_lsb_loc', 'iceil_log2', 'cost_add', 'dais_interp_run', 'device_info', 'plan', 'set_stream', 'set_group_size', 'set_accounting',
 ]  # fmt: skip

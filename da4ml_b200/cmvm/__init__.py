@@ -5,12 +5,14 @@ GPU-side additions for many independent matrices, ``solve_sweep`` for one matrix
 ``solve_sweep_batch`` for many matrices under many option sets, ``network_front`` for the cheapest per-layer choice of a
 chain of layers under a latency budget, and ``chain_front`` for the same with each layer solved under the output latencies
 of the design before it (the designs and latencies a traced model gets).  ``solve``'s ``seed`` keyword picks the
-tie-break order of the greedy pair selection (0 = the reference's), and ``solve_best_of`` keeps the cheapest of many seeds."""
+tie-break order of the greedy pair selection (0 = the reference's), and ``solve_best_of`` keeps the cheapest of many seeds.
+``price_pipelined`` prices designs as they will be pipelined under a latency cutoff: clock stages, register bits and the
+tracer's latencies."""
 
 from typing import TypedDict
 
-from .._binary import (ChainFront, NetworkFront, SweepResult, chain_front, kernel_decompose, network_front, solve, solve_batch, solve_best_of, solve_sweep,
-                       solve_sweep_batch)  # fmt: skip
+from .._binary import (ChainFront, NetworkFront, PipelinePrice, SweepResult, chain_front, kernel_decompose, network_front, price_pipelined, solve, solve_batch,
+                       solve_best_of, solve_sweep, solve_sweep_batch)  # fmt: skip
 from ..batching import CmvmCall, SolveBatcher, solve_calls
 from ..types import CombLogic, Op, Pipeline, QInterval
 
@@ -32,4 +34,4 @@ solver_options_t = TypedDict(
     total=False,
 )
 
-__all__ = ['solve', 'solve_batch', 'solve_best_of', 'solve_sweep', 'solve_sweep_batch', 'SweepResult', 'network_front', 'NetworkFront', 'chain_front', 'ChainFront', 'solve_calls', 'CmvmCall', 'SolveBatcher', 'kernel_decompose', 'QInterval', 'Op', 'CombLogic', 'Pipeline', 'solver_options_t']
+__all__ = ['solve', 'solve_batch', 'solve_best_of', 'solve_sweep', 'solve_sweep_batch', 'SweepResult', 'network_front', 'NetworkFront', 'chain_front', 'ChainFront', 'price_pipelined', 'PipelinePrice', 'solve_calls', 'CmvmCall', 'SolveBatcher', 'kernel_decompose', 'QInterval', 'Op', 'CombLogic', 'Pipeline', 'solver_options_t']

@@ -8,6 +8,7 @@
 // cmvm_decompose.cuh; nothing here falls back to the CPU.
 #include "dais_program.cuh"
 #include "host_solve.cuh"
+#include "pipeline_price.cuh"
 
 namespace da {
 
@@ -578,6 +579,157 @@ int da4ml_sweep_front(const float *cost, const float *latency_max, int64_t n, in
         return DA4ML_E_INVALID;
     pareto_front(cost, latency_max, n, front);
     return DA4ML_OK;
+}
+
+int da4ml_pipeline_price(
+    int64_t n_designs, const int64_t *n_stages, const int64_t *stage_meta, const int64_t *inp_shifts, const int64_t *out_idxs, const int64_t *out_shifts,
+    const int64_t *out_negs, const int64_t *ops_i, const float *ops_f, const double *latencies, const double *cutoffs, int64_t n_cutoffs, int retiming,
+    int32_t *status, int64_t *stages, int64_t *reg_bits, double *latency_max, double *cutoff_out, double *out_latency, double profile[2]
+) {
+    return guarded([&] {
+        if (n_designs < 1 || n_designs > (1 << 24) || !n_stages || !stage_meta)
+            throw ApiError(DA4ML_E_INVALID, "pipeline_price: n_designs must be positive and the design arrays non-null");
+        if (n_cutoffs < 1 || n_cutoffs > (1 << 16) || !cutoffs)
+            throw ApiError(DA4ML_E_INVALID, "pipeline_price: at least one latency cutoff is needed");
+        if (!status || !stages || !reg_bits || !latency_max || !cutoff_out)
+            throw ApiError(DA4ML_E_INVALID, "pipeline_price: an output array is null");
+        if (n_designs * n_cutoffs > (1 << 24))
+            throw ApiError(DA4ML_E_INVALID, "pipeline_price: too many (design, cutoff) tasks");
+        for (int64_t j = 0; j < n_cutoffs; ++j)
+            if (!(cutoffs[j] > 0) || !std::isfinite(cutoffs[j]))
+                throw ApiError(DA4ML_E_INVALID, "pipeline_price: latency cutoff " + std::to_string(j) + " is " + std::to_string(cutoffs[j]) +
+                                                    "; it must be positive and finite (cutoff 0 is the unpipelined design the solver reports)");
+        // host preparation of every design (all argument checks happen here, before the device is touched)
+        std::vector<PpPrepared> prep(n_designs);
+        std::vector<int64_t> lat_off(n_designs);
+        int64_t s0 = 0, o_in = 0, o_out = 0, o_ops = 0, lat_n = 0;
+        for (int64_t d = 0; d < n_designs; ++d) {
+            if (n_stages[d] < 1 || n_stages[d] > (1 << 16))
+                throw ApiError(DA4ML_E_INVALID, "pipeline_price: design " + std::to_string(d) + " has " + std::to_string(n_stages[d]) + " stages");
+            std::vector<PpStageIn> st(n_stages[d]);
+            for (int64_t k = 0; k < n_stages[d]; ++k, ++s0) {
+                const int64_t *m = stage_meta + 5 * s0;
+                PpStageIn &S = st[k];
+                S.n_in = m[0], S.n_out = m[1], S.n_ops = m[2], S.carry_size = m[3], S.adder_size = m[4];
+                if (S.n_in < 0 || S.n_out < 0 || S.n_ops < 0)
+                    throw ApiError(DA4ML_E_INVALID, "pipeline_price: design " + std::to_string(d) + " stage " + std::to_string(k) + " has a negative size");
+                S.inp_shifts = inp_shifts ? inp_shifts + o_in : nullptr;
+                S.out_idxs = out_idxs ? out_idxs + o_out : nullptr;
+                S.out_shifts = out_shifts ? out_shifts + o_out : nullptr;
+                S.out_negs = out_negs ? out_negs + o_out : nullptr;
+                S.ops_i = ops_i ? ops_i + 4 * o_ops : nullptr;
+                S.ops_f = ops_f ? ops_f + 5 * o_ops : nullptr;
+                o_in += S.n_in, o_out += S.n_out, o_ops += S.n_ops;
+            }
+            try {
+                prep[d] = pp_prepare(st.data(), n_stages[d]);
+            }
+            catch (const std::invalid_argument &e) {
+                throw ApiError(DA4ML_E_INVALID, std::string(e.what()) + " (design " + std::to_string(d) + ")");
+            }
+            lat_off[d] = lat_n;
+            lat_n += prep[d].n_in;
+        }
+        if (latencies)
+            for (int64_t i = 0; i < lat_n; ++i)
+                if (!std::isfinite(latencies[i]) || latencies[i] < 0)
+                    throw ApiError(DA4ML_E_INVALID, "pipeline_price: input latency " + std::to_string(i) + " is not a finite non-negative number");
+        init_device();
+        // one device buffer: the prepared designs, the input latencies, per task its workspace and output latencies,
+        // the task list and the results
+        const int64_t n_tasks = n_designs * n_cutoffs;
+        Carver c;
+        std::vector<size_t> o_add(n_designs), o_lvl(n_designs), o_bits(n_designs), o_onode(n_designs), o_ws(n_tasks), o_olat(n_tasks);
+        for (int64_t d = 0; d < n_designs; ++d) {
+            o_add[d] = c.take(sizeof(PpAdd) * prep[d].adds.size());
+            o_lvl[d] = c.take(sizeof(int) * prep[d].lvl_begin.size());
+            o_bits[d] = c.take(sizeof(int) * prep[d].node_bits.size());
+            o_onode[d] = c.take(sizeof(int) * prep[d].out_node.size());
+        }
+        const size_t o_desc = c.take(sizeof(PpDesign) * n_designs), o_lat = c.take(sizeof(double) * lat_n);
+        for (int64_t t = 0; t < n_tasks; ++t) {
+            const PpPrepared &P = prep[t / n_cutoffs];
+            o_ws[t] = c.take((sizeof(double) + sizeof(int)) * P.n_nodes);
+            o_olat[t] = c.take(out_latency ? sizeof(double) * P.n_out : 0);
+        }
+        const size_t o_task = c.take(sizeof(PpTask) * n_tasks), o_res = c.take(sizeof(PpResult) * n_tasks);
+        static DevBuf buf;
+        buf.ensure(c.off, false);
+        char *b = (char *)buf.p;
+        std::vector<PpDesign> desc(n_designs);
+        auto up = [&](size_t off, const void *src, size_t bytes) {
+            if (bytes)
+                CK(cudaMemcpyAsync(b + off, src, bytes, cudaMemcpyHostToDevice, g_stream));
+        };
+        for (int64_t d = 0; d < n_designs; ++d) {
+            const PpPrepared &P = prep[d];
+            up(o_add[d], P.adds.data(), sizeof(PpAdd) * P.adds.size());
+            up(o_lvl[d], P.lvl_begin.data(), sizeof(int) * P.lvl_begin.size());
+            up(o_bits[d], P.node_bits.data(), sizeof(int) * P.node_bits.size());
+            up(o_onode[d], P.out_node.data(), sizeof(int) * P.out_node.size());
+            desc[d] = PpDesign{(const PpAdd *)(b + o_add[d]), (const int *)(b + o_lvl[d]), (const int *)(b + o_bits[d]), (const int *)(b + o_onode[d]),
+                               P.n_in, P.n_nodes, (int)P.adds.size(), (int)P.lvl_begin.size() - 1, P.n_out, P.adder_size, P.carry_size, 0, P.out_bits};
+        }
+        up(o_desc, desc.data(), sizeof(PpDesign) * n_designs);
+        if (latencies)
+            up(o_lat, latencies, sizeof(double) * lat_n);
+        Timing tm;
+        auto run = [&](const std::vector<PpRequest> &req, std::vector<PpResult> &res) {
+            std::vector<PpTask> tasks(req.size());
+            for (size_t k = 0; k < req.size(); ++k) {
+                const PpRequest &q = req[k];
+                const PpPrepared &P = prep[q.design];
+                PpTask &T = tasks[k];
+                T.design = q.design;
+                T.pad = 0;
+                T.cutoff = q.cutoff;
+                T.in_lat = latencies && !q.zero_latency ? (const double *)(b + o_lat) + lat_off[q.design] : nullptr;
+                T.lat = (double *)(b + o_ws[q.slot]);
+                T.last_use = (int *)(T.lat + P.n_nodes);
+                T.out_lat = out_latency && !q.zero_latency ? (double *)(b + o_olat[q.slot]) : nullptr;
+            }
+            up(o_task, tasks.data(), sizeof(PpTask) * tasks.size());
+            tm.begin();
+            pipeline_price_kernel<<<(unsigned)tasks.size(), 256, 0, g_stream>>>((const PpDesign *)(b + o_desc), (const PpTask *)(b + o_task), (PpResult *)(b + o_res));
+            CK(cudaGetLastError());
+            tm.end(1);
+            res.resize(req.size());
+            CK(cudaMemcpyAsync(res.data(), b + o_res, sizeof(PpResult) * req.size(), cudaMemcpyDeviceToHost, g_stream));
+            CK(cudaStreamSynchronize(g_stream));
+        };
+        bool first = true;
+        auto run_first = [&](const std::vector<PpRequest> &req, std::vector<PpResult> &res) {
+            run(req, res);
+            if (first && out_latency) { // the traced output latencies of the first pass (the tasks' own latencies)
+                int64_t off = 0;
+                for (int64_t t = 0; t < n_tasks; ++t) {
+                    const int n_out = prep[t / n_cutoffs].n_out;
+                    if (n_out)
+                        CK(cudaMemcpyAsync(out_latency + off, b + o_olat[t], sizeof(double) * n_out, cudaMemcpyDeviceToHost, g_stream));
+                    off += n_out;
+                }
+                CK(cudaStreamSynchronize(g_stream));
+                for (int64_t t = 0, o = 0; t < n_tasks; ++t)
+                    for (int k = 0; k < prep[t / n_cutoffs].n_out; ++k, ++o)
+                        if (res[t].status != PP_OK)
+                            out_latency[o] = nan("");
+            }
+            first = false;
+        };
+        const std::vector<PpAnswer> ans = pp_price((int)n_designs, cutoffs, (int)n_cutoffs, retiming != 0, run_first);
+        tm.collect();
+        for (int64_t t = 0; t < n_tasks; ++t) {
+            status[t] = ans[t].status;
+            stages[t] = ans[t].stages;
+            reg_bits[t] = ans[t].reg_bits;
+            latency_max[t] = ans[t].latency_max;
+            cutoff_out[t] = ans[t].status == PP_OK ? ans[t].cutoff : nan("");
+        }
+        if (profile) {
+            profile[0] = tm.device_ms;
+            profile[1] = (double)tm.launches;
+        }
+    });
 }
 
 void da4ml_pipeline_free(da4ml_pipeline_t *p) { delete p; }

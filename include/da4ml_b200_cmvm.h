@@ -213,6 +213,31 @@ int64_t da4ml_pipeline_launches(const da4ml_pipeline_t *p);
  * algorithmic_bytes (all solve_single jobs of the call, exact in accounting mode), 0, 0, 0}. */
 int da4ml_pipeline_profile(const da4ml_pipeline_t *p, double out[8]);
 
+/* ---- pipelined pricing ----------------------------------------------------------------------------
+ * Price designs (solver results) as they will be pipelined under latency cutoffs: for every (design d, cutoff j), what
+ * the reference computes by replaying d's stages through its symbolic tracer under HWConfig(adder_size, carry_size, c)
+ * with the inputs at d's input latencies, gathering the result with comb_trace (dead ops dropped) and splitting it with
+ * to_pipeline(comb, c, retiming=0); with retiming = 1, what retime_pipeline then keeps (every re-trace has its inputs at
+ * latency 0, as the reference's re-trace of a split has them).
+ * Designs are given as flat per-stage arrays, the stages of all designs concatenated in order: n_stages[n_designs];
+ * stage_meta [total stages][5] = {n_in, n_out, n_ops, carry_size, adder_size} (da4ml_pipeline_stage_meta); inp_shifts,
+ * out_idxs, out_shifts, out_negs, ops_i [.,4], ops_f [.,5] concatenated in the layout of da4ml_pipeline_stage_copy.
+ * latencies: per design its first stage's n_in input latencies, concatenated (NULL: zeros).  cutoffs[n_cutoffs] > 0.
+ * Outputs [n_designs][n_cutoffs]: status (0 ok, 1 an adder is slower than the cutoff -- the tracer's AssertionError,
+ * 2 not supported -- a constant intermediate value), stages (len of the split), reg_bits (Pipeline.reg_bits of the
+ * split), latency_max (the traced output latencies' maximum), cutoff_out (the cutoff retiming settled on; the cutoff
+ * itself without retiming); out_latency (NULL to skip) [n_designs][n_cutoffs][n_out of the design] the traced output
+ * latencies (0.0 for a dead column).  Not ok: stages = reg_bits = -1, latencies NaN.  profile (NULL to skip) =
+ * {device_ms, launches}.  Arguments are checked on the host before any device call: shapes, opcodes other than -1/0/1,
+ * operands and cutoffs <= 0 give DA4ML_E_INVALID. */
+int da4ml_pipeline_price(
+    int64_t n_designs, const int64_t *n_stages, const int64_t *stage_meta, const int64_t *inp_shifts,
+    const int64_t *out_idxs, const int64_t *out_shifts, const int64_t *out_negs, const int64_t *ops_i,
+    const float *ops_f, const double *latencies, const double *cutoffs, int64_t n_cutoffs, int retiming,
+    int32_t *status, int64_t *stages, int64_t *reg_bits, double *latency_max, double *cutoff_out,
+    double *out_latency, double profile[2]
+);
+
 /* ---- DAIS interpreter (SURVEY 8f N2) ----------------------------------------------------------------
  * Replaces `run_interp` of the reference's second native module (dais/bindings.cc:30-131 -> DAISInterpreter.cc) for
  * every DAIS program: all opcodes of DAISInterpreter::exec_ops and lookup tables.  Programs are the int32 words of
