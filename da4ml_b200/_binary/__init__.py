@@ -88,6 +88,11 @@ _L.da4ml_cmvm_cost_add.argtypes = [_f32p, _f32p, C.c_int64, C.c_int, C.c_int, C.
 _f64p = C.POINTER(C.c_double)
 _L.da4ml_pipeline_price.argtypes = [C.c_int64, _i64p, _i64p, _i64p, _i64p, _i64p, _i64p, _i64p, _f32p, _f64p, _f64p, C.c_int64, C.c_int, _i32p, _i64p, _i64p, _f64p,
                                     _f64p, _f64p, _f64p]  # fmt: skip
+_L.da4ml_pipeline_split.argtypes = [*_L.da4ml_pipeline_price.argtypes, C.POINTER(_vp)]
+_L.da4ml_split_info.argtypes = [_vp, C.c_int64, _i64p]
+_L.da4ml_split_copy.argtypes = [_vp, C.c_int64, _i64p, _i64p, _i64p, _i64p, _i64p, _f64p]
+_L.da4ml_split_free.argtypes = [_vp]
+_L.da4ml_split_free.restype = None
 
 EXPORTED_SYMBOLS = [
     'da4ml_cmvm_last_error', 'da4ml_cmvm_device_info', 'da4ml_cmvm_set_stream', 'da4ml_cmvm_set_group_size',
@@ -101,6 +106,7 @@ EXPORTED_SYMBOLS = [
     'da4ml_dais_program_free', 'da4ml_dais_program_profile', 'da4ml_dais_program_dump', 'da4ml_cmvm_solve_sweep', 'da4ml_cmvm_solve_sweep_batch', 'da4ml_sweep_counts',
     'da4ml_sweep_profile', 'da4ml_sweep_summary', 'da4ml_sweep_pipeline', 'da4ml_sweep_free', 'da4ml_sweep_front',
     'da4ml_cmvm_solve_seeded', 'da4ml_cmvm_solve_single_seeded', 'da4ml_cmvm_solve_sweep_batch_seeded', 'da4ml_pipeline_price',
+    'da4ml_pipeline_split', 'da4ml_split_info', 'da4ml_split_copy', 'da4ml_split_free',
 ]  # fmt: skip
 
 COUNTER_NAMES = ['status', 'n_ops', 'T', 'sum_F', 'sum_R', 'F0', 'R0', 'D_final', 'F_max', 'compactions', 'D0', 'n_bits', 'group_ctas',
@@ -520,16 +526,18 @@ class SweepResult:
             call['seed'] = int(s['seed'])
         return call
 
-    def pipelined(self, latency_cutoff, retiming: bool = True, pricer=None) -> 'PipelinePrice':
+    def pipelined(self, latency_cutoff, retiming: bool = True, pricer=None, keep_split: bool = False) -> 'PipelinePrice':
         """``price_pipelined`` of every candidate whose op tables were kept, under the sweep's own input latencies, in one
         call.  The arrays are aligned with ``candidates`` (``[len(self), n_cutoffs]``); a candidate that was not kept has
         status -1, ``stages`` / ``reg_bits`` -1 and NaN latencies.  Only the winners and the front are kept unless the
         sweep ran with ``keep_all=True``, which is needed to price every candidate.  ``pricer`` stands in for
-        ``price_pipelined``."""
+        ``price_pipelined``.  ``keep_split=True``: ``split(i, j)`` gives candidate ``i``'s register stages under cutoff
+        ``j``."""
         kept = np.flatnonzero(self.candidates['kept'])
         lat = self._call['latencies']
+        kw = dict(keep_split=True) if keep_split else {}
         pr = (price_pipelined if pricer is None else pricer)([self.raw(int(i)) for i in kept], latency_cutoff, latencies=None if lat is None else [lat] * kept.size,
-                                                             retiming=retiming)  # fmt: skip
+                                                             retiming=retiming, **kw)  # fmt: skip
         return pr._scatter(kept, len(self))
 
 
@@ -879,11 +887,33 @@ class PipelinePrice:
     ``reg_bits`` (``Pipeline.reg_bits`` of the split), ``latency_max`` (the traced output latencies' maximum, float64)
     and ``cutoff`` (the cutoff retiming settled on, or the cutoff itself without retiming), ``cutoffs`` (the cutoffs
     asked for), and ``out_latency(d, j)``: design ``d``'s traced output latencies under cutoff ``j``.  A task that is not
-    ok has ``stages`` and ``reg_bits`` -1 and NaN latencies.  ``profile``: the call's device time and launches."""
+    ok has ``stages`` and ``reg_bits`` -1 and NaN latencies.  ``profile``: the call's device time and launches (with
+    ``keep_split``, also ``split_launches`` and ``split_bytes``, the bytes of op tables copied back).  ``split(d, j)``:
+    design ``d``'s register stages under cutoff ``j`` when the call kept them."""
 
-    def __init__(self, status, stages, reg_bits, latency_max, cutoff, cutoffs, out_lat, profile):
+    def __init__(self, status, stages, reg_bits, latency_max, cutoff, cutoffs, out_lat, profile, splits=None):
         self.status, self.stages, self.reg_bits, self.latency_max, self.cutoff = status, stages, reg_bits, latency_max, cutoff
         self.cutoffs, self._out_lat, self.profile = cutoffs, out_lat, profile
+        self._splits = splits  # None: not kept; else per design None (not priced) or per cutoff (status, tables)
+
+    def split(self, d: int, j: int = 0) -> list[dict]:
+        """The register stages of design ``d`` under cutoff ``j``: what the reference's ``to_pipeline(comb, c, retiming)``
+        returns for the task -- without retiming the split of the trace under the design's input latencies; with it,
+        ``retime_pipeline``'s (the first split when no bisection round succeeded, else the last successful round's, at
+        cutoff ``self.cutoff[d, j]`` with every input at latency 0).  Stage dicts in the layout of ``RawPipeline.stages``
+        (``ops_f`` float64), for ``emit.verilog_pipeline_logic_gen`` / ``types.pipeline_from_arrays``.  ``ValueError``
+        when the splits were not kept, the task is not ok, or the reference's ``to_pipeline`` raises on it (a ``KeyError``:
+        a stage would have no op or no output, as when every input arrives after the first stage)."""
+        d, j = int(d), int(j)
+        if self._splits is None or self._splits[d] is None:
+            raise ValueError(f'the split of design {d} was not kept (price_pipelined(..., keep_split=True) keeps it)')
+        if int(self.status[d, j]) != 0:
+            raise ValueError(f'design {d} under cutoff {float(self.cutoffs[j])} is not ok ({PRICE_STATUS[int(self.status[d, j])]}): it has no split')
+        code, tables = self._splits[d][j]
+        if code == 2:
+            raise ValueError(f"design {d} under cutoff {float(self.cutoffs[j])}: the reference's to_pipeline raises KeyError on this task "
+                             '(a stage would have no op or no output, as when every input arrives after the first stage)')  # fmt: skip
+        return _split_stages(*tables)
 
     def __len__(self):
         return len(self.status)
@@ -909,10 +939,46 @@ class PipelinePrice:
             return out
 
         out_lat = [None] * n
+        splits = None if self._splits is None else [None] * n
         for k, r in enumerate(np.asarray(rows, np.int64).tolist()):
             out_lat[r] = self._out_lat[k]
+            if splits is not None:
+                splits[r] = self._splits[k]
         return PipelinePrice(put(self.status, -1), put(self.stages, -1), put(self.reg_bits, -1), put(self.latency_max, np.nan), put(self.cutoff, np.nan),
-                             self.cutoffs, out_lat, self.profile)  # fmt: skip
+                             self.cutoffs, out_lat, self.profile, splits)  # fmt: skip
+
+
+def _split_stages(meta, outs, shifts, negs, ops_i, ops_f, adder_size, carry_size) -> list[dict]:
+    """Stage dicts (fresh arrays) of one split from its concatenated tables."""
+    stages, o, r = [], 0, 0
+    for n_in, n_out, n_ops in meta.tolist():
+        stages.append(dict(shape=(n_in, n_out), inp_shifts=np.zeros(n_in, np.int64), out_idxs=outs[o : o + n_out].copy(), out_shifts=shifts[o : o + n_out].copy(),
+                           out_negs=negs[o : o + n_out].astype(bool), ops_i=ops_i[r : r + n_ops].copy(), ops_f=ops_f[r : r + n_ops].copy(), adder_size=adder_size,
+                           carry_size=carry_size))  # fmt: skip
+        o, r = o + n_out, r + n_ops
+    return stages
+
+
+def _take_splits(designs, m, info, copy) -> list:
+    """Per design, per cutoff (status, tables) of the splits a call kept; ``info(t, out[4])`` / ``copy(t, ...)`` read task
+    ``t`` (``da4ml_split_info`` / ``da4ml_split_copy`` or the CPU harness's)."""
+    q = np.zeros(4, np.int64)
+    out = []
+    for d, stages in enumerate(designs):
+        row = []
+        for j in range(m):
+            info(d * m + j, q)
+            code, n_st, n_rows, n_outs = (int(v) for v in q)
+            if code != 0:
+                row.append((code, None))
+                continue
+            meta = np.zeros((n_st, 3), np.int64)
+            outs, shifts, negs = np.zeros(n_outs, np.int64), np.zeros(n_outs, np.int64), np.zeros(n_outs, np.int64)
+            ops_i, ops_f = np.zeros((n_rows, 4), np.int64), np.zeros((n_rows, 5), np.float64)
+            copy(d * m + j, meta, outs, shifts, negs, ops_i, ops_f)
+            row.append((0, (meta, outs, shifts, negs, ops_i, ops_f, int(stages[0]['adder_size']), int(stages[0]['carry_size']))))
+        out.append(row)
+    return out
 
 
 def _design_stages(design) -> list[dict]:
@@ -952,7 +1018,7 @@ def _price_args(designs, latency_cutoff, latencies) -> dict:
                 ops_f=ops_f)  # fmt: skip
 
 
-def price_pipelined(designs, latency_cutoff, latencies=None, retiming: bool = True) -> PipelinePrice:
+def price_pipelined(designs, latency_cutoff, latencies=None, retiming: bool = True, keep_split: bool = False) -> PipelinePrice:
     """Price designs as they will be pipelined, on the GPU: for every design and every cutoff ``c`` what the reference gets
     by replaying the design through its tracer under ``HWConfig(adder_size, carry_size, c)`` with its inputs at
     ``latencies``, gathering it with ``comb_trace`` and splitting it with ``to_pipeline(comb, c, retiming)``.
@@ -965,7 +1031,12 @@ def price_pipelined(designs, latency_cutoff, latencies=None, retiming: bool = Tr
 
     A task that is not ``ok`` (an adder slower than the cutoff, a constant intermediate value) does not raise: it is
     reported in ``status``, so one slow adder does not fail a sweep.  Argument errors raise ``ValueError`` before any
-    device call."""
+    device call.
+
+    ``keep_split=True`` also builds every ok task's register stages on the GPU (two more launches, after pricing and the
+    bisection) and keeps them: ``split(d, j)``.  A split is the reference's only where pricing is: the retimed split
+    re-traces with every input at latency 0, which is the reference's re-trace when every input is in the first stage.
+    The other arrays are the same with and without it."""
     pk = _price_args(designs, latency_cutoff, latencies)
     designs, cut, lat = pk['designs'], pk['cutoffs'], pk['latencies']
     n, m = len(designs), cut.size
@@ -974,14 +1045,27 @@ def price_pipelined(designs, latency_cutoff, latencies=None, retiming: bool = Tr
     stg, rb = np.zeros(n * m, np.int64), np.zeros(n * m, np.int64)
     lm, co = np.zeros(n * m), np.zeros(n * m)
     ol = np.zeros(sum(n_out) * m)
-    prof = np.zeros(2)
+    prof = np.zeros(4 if keep_split else 2)
     f64 = lambda a: a.ctypes.data_as(_f64p) if a is not None else None  # noqa: E731
-    _check(_L.da4ml_pipeline_price(n, *[_ip(pk[k]) for k in ('n_stages', 'meta', 'inp_shifts', 'out_idxs', 'out_shifts', 'out_negs', 'ops_i')], _fp(pk['ops_f']),
-                                   f64(lat), f64(cut), m, int(bool(retiming)), st_.ctypes.data_as(_i32p), _ip(stg), _ip(rb), f64(lm), f64(co), f64(ol), f64(prof)))  # fmt: skip
+    args = [n, *[_ip(pk[k]) for k in ('n_stages', 'meta', 'inp_shifts', 'out_idxs', 'out_shifts', 'out_negs', 'ops_i')], _fp(pk['ops_f']), f64(lat), f64(cut), m,
+            int(bool(retiming)), st_.ctypes.data_as(_i32p), _ip(stg), _ip(rb), f64(lm), f64(co), f64(ol), f64(prof)]  # fmt: skip
+    splits = None
+    if keep_split:
+        h = _vp()
+        _check(_L.da4ml_pipeline_split(*args, C.byref(h)))
+        try:
+            f = lambda a: a.ctypes.data_as(_f64p if a.dtype == np.float64 else _i64p)  # noqa: E731
+            splits = _take_splits(designs, m, lambda t, q: _check(_L.da4ml_split_info(h, t, _ip(q))), lambda t, *a: _check(_L.da4ml_split_copy(h, t, *map(f, a))))
+        finally:
+            _L.da4ml_split_free(h)
+    else:
+        _check(_L.da4ml_pipeline_price(*args))
     edges = np.concatenate([[0], np.cumsum(np.asarray(n_out, np.int64) * m)])
     out_lat = [ol[edges[d] : edges[d + 1]].reshape(m, n_out[d]) for d in range(n)]
-    return PipelinePrice(st_.reshape(n, m), stg.reshape(n, m), rb.reshape(n, m), lm.reshape(n, m), co.reshape(n, m), cut, out_lat,
-                         dict(device_ms=float(prof[0]), launches=int(prof[1])))  # fmt: skip
+    profile = dict(device_ms=float(prof[0]), launches=int(prof[1]))
+    if keep_split:
+        profile.update(split_launches=int(prof[2]), split_bytes=int(prof[3]))
+    return PipelinePrice(st_.reshape(n, m), stg.reshape(n, m), rb.reshape(n, m), lm.reshape(n, m), co.reshape(n, m), cut, out_lat, profile, splits)
 
 
 def csd_decompose(inp, center=True):

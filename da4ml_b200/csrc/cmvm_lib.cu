@@ -8,7 +8,7 @@
 // cmvm_decompose.cuh; nothing here falls back to the CPU.
 #include "dais_program.cuh"
 #include "host_solve.cuh"
-#include "pipeline_price.cuh"
+#include "pipeline_split.cuh"
 
 namespace da {
 
@@ -53,6 +53,9 @@ struct da4ml_pipeline {
     std::unique_ptr<PipelineImpl> impl;
 };
 
+struct da4ml_split {
+    PsResult r;
+};
 struct da4ml_sweep {
     std::unique_ptr<SweepImpl> impl;
 };
@@ -581,10 +584,46 @@ int da4ml_sweep_front(const float *cost, const float *latency_max, int64_t n, in
     return DA4ML_OK;
 }
 
-int da4ml_pipeline_price(
+namespace {
+// ps_split's device: the call's three cached buffers, launches on the library stream with CUDA-event timing
+struct CudaSplitDev {
+    int threads = 256;
+    Timing *tm = nullptr;
+    size_t bytes_down = 0;
+    char *buffer(int which, size_t bytes) {
+        static DevBuf bufs[3];
+        bufs[which].ensure(bytes, false);
+        return (char *)bufs[which].p;
+    }
+    void up(void *dst, const void *src, size_t bytes) {
+        if (bytes)
+            CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, g_stream));
+    }
+    void down(void *dst, const void *src, size_t bytes) {
+        if (bytes)
+            CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, g_stream));
+        CK(cudaStreamSynchronize(g_stream));
+    }
+    void count(const PsDesign *d, const PsTask *t, int n) {
+        tm->begin();
+        pipeline_split_kernel<<<(unsigned)n, threads, 0, g_stream>>>(d, t);
+        CK(cudaGetLastError());
+        tm->end(1);
+    }
+    void write(const PsDesign *d, const PsTask *t, int n) {
+        tm->begin();
+        pipeline_split_write_kernel<<<(unsigned)n, threads, 0, g_stream>>>(d, t);
+        CK(cudaGetLastError());
+        tm->end(1);
+    }
+};
+} // namespace
+
+// da4ml_pipeline_price, and with `split` non-null da4ml_pipeline_split (profile then has 4 entries)
+static int pipeline_price_impl(
     int64_t n_designs, const int64_t *n_stages, const int64_t *stage_meta, const int64_t *inp_shifts, const int64_t *out_idxs, const int64_t *out_shifts,
     const int64_t *out_negs, const int64_t *ops_i, const float *ops_f, const double *latencies, const double *cutoffs, int64_t n_cutoffs, int retiming,
-    int32_t *status, int64_t *stages, int64_t *reg_bits, double *latency_max, double *cutoff_out, double *out_latency, double profile[2]
+    int32_t *status, int64_t *stages, int64_t *reg_bits, double *latency_max, double *cutoff_out, double *out_latency, double *profile, da4ml_split_t **split
 ) {
     return guarded([&] {
         if (n_designs < 1 || n_designs > (1 << 24) || !n_stages || !stage_meta)
@@ -601,6 +640,7 @@ int da4ml_pipeline_price(
                                                     "; it must be positive and finite (cutoff 0 is the unpipelined design the solver reports)");
         // host preparation of every design (all argument checks happen here, before the device is touched)
         std::vector<PpPrepared> prep(n_designs);
+        std::vector<PpSplitInfo> info(split ? n_designs : 0);
         std::vector<int64_t> lat_off(n_designs);
         int64_t s0 = 0, o_in = 0, o_out = 0, o_ops = 0, lat_n = 0;
         for (int64_t d = 0; d < n_designs; ++d) {
@@ -622,7 +662,7 @@ int da4ml_pipeline_price(
                 o_in += S.n_in, o_out += S.n_out, o_ops += S.n_ops;
             }
             try {
-                prep[d] = pp_prepare(st.data(), n_stages[d]);
+                prep[d] = pp_prepare(st.data(), n_stages[d], split ? &info[d] : nullptr);
             }
             catch (const std::invalid_argument &e) {
                 throw ApiError(DA4ML_E_INVALID, std::string(e.what()) + " (design " + std::to_string(d) + ")");
@@ -717,6 +757,20 @@ int da4ml_pipeline_price(
             first = false;
         };
         const std::vector<PpAnswer> ans = pp_price((int)n_designs, cutoffs, (int)n_cutoffs, retiming != 0, run_first);
+        std::unique_ptr<da4ml_split> sp_out;
+        int64_t split_launches = 0;
+        size_t split_bytes = 0;
+        if (split) { // every ok task's split, at the (cutoff, latencies) it comes from
+            std::vector<PsPrep> sp(n_designs);
+            for (int64_t d = 0; d < n_designs; ++d)
+                sp[d] = ps_prepare(prep[d], info[d]);
+            CudaSplitDev dev;
+            dev.tm = &tm;
+            sp_out.reset(new da4ml_split{ps_split(prep, sp, desc, ans, cutoffs, n_cutoffs, retiming != 0, latencies, latencies ? (const double *)(b + o_lat) : nullptr,
+                                                  lat_off, dev)});  // fmt: skip
+            split_launches = sp_out->r.launches;
+            split_bytes = sp_out->r.tables.size();
+        }
         tm.collect();
         for (int64_t t = 0; t < n_tasks; ++t) {
             status[t] = ans[t].status;
@@ -728,9 +782,61 @@ int da4ml_pipeline_price(
         if (profile) {
             profile[0] = tm.device_ms;
             profile[1] = (double)tm.launches;
+            if (split)
+                profile[2] = (double)split_launches, profile[3] = (double)split_bytes;
         }
+        if (split)
+            *split = sp_out.release();
     });
 }
+
+int da4ml_pipeline_price(
+    int64_t n_designs, const int64_t *n_stages, const int64_t *stage_meta, const int64_t *inp_shifts, const int64_t *out_idxs, const int64_t *out_shifts,
+    const int64_t *out_negs, const int64_t *ops_i, const float *ops_f, const double *latencies, const double *cutoffs, int64_t n_cutoffs, int retiming,
+    int32_t *status, int64_t *stages, int64_t *reg_bits, double *latency_max, double *cutoff_out, double *out_latency, double profile[2]
+) {
+    return pipeline_price_impl(n_designs, n_stages, stage_meta, inp_shifts, out_idxs, out_shifts, out_negs, ops_i, ops_f, latencies, cutoffs, n_cutoffs, retiming, status,
+                               stages, reg_bits, latency_max, cutoff_out, out_latency, profile, nullptr);
+}
+
+int da4ml_pipeline_split(
+    int64_t n_designs, const int64_t *n_stages, const int64_t *stage_meta, const int64_t *inp_shifts, const int64_t *out_idxs, const int64_t *out_shifts,
+    const int64_t *out_negs, const int64_t *ops_i, const float *ops_f, const double *latencies, const double *cutoffs, int64_t n_cutoffs, int retiming,
+    int32_t *status, int64_t *stages, int64_t *reg_bits, double *latency_max, double *cutoff_out, double *out_latency, double profile[4], da4ml_split_t **out
+) {
+    if (!out)
+        return guarded([] { throw ApiError(DA4ML_E_INVALID, "pipeline_split: the handle pointer is null"); });
+    *out = nullptr;
+    return pipeline_price_impl(n_designs, n_stages, stage_meta, inp_shifts, out_idxs, out_shifts, out_negs, ops_i, ops_f, latencies, cutoffs, n_cutoffs, retiming, status,
+                               stages, reg_bits, latency_max, cutoff_out, out_latency, profile, out);
+}
+
+int da4ml_split_info(const da4ml_split_t *s, int64_t task, int64_t out[4]) {
+    return guarded([&] {
+        if (!s || !out)
+            throw ApiError(DA4ML_E_INVALID, "split_info: the handle or the output array is null");
+        if (task < 0 || task >= (int64_t)s->r.tasks.size())
+            throw ApiError(DA4ML_E_INVALID, "split_info: task " + std::to_string(task) + " is out of range [0, " + std::to_string(s->r.tasks.size()) + ")");
+        ps_info(s->r, task, out);
+    });
+}
+
+int da4ml_split_copy(const da4ml_split_t *s, int64_t task, int64_t *stage_meta, int64_t *out_idxs, int64_t *out_shifts, int64_t *out_negs, int64_t *ops_i, double *ops_f) {
+    return guarded([&] {
+        if (!s)
+            throw ApiError(DA4ML_E_INVALID, "split_copy: the handle is null");
+        if (task < 0 || task >= (int64_t)s->r.tasks.size())
+            throw ApiError(DA4ML_E_INVALID, "split_copy: task " + std::to_string(task) + " is out of range [0, " + std::to_string(s->r.tasks.size()) + ")");
+        const PsSplit &S = s->r.tasks[task];
+        if (S.status != PS_SPLIT)
+            throw ApiError(DA4ML_E_INVALID, "split_copy: task " + std::to_string(task) + " has no split (da4ml_split_info status " + std::to_string(S.status) + ")");
+        if (!stage_meta || !out_idxs || !out_shifts || !out_negs || (S.n_rows && (!ops_i || !ops_f)))
+            throw ApiError(DA4ML_E_INVALID, "split_copy: an output array is null");
+        ps_copy(s->r, task, stage_meta, out_idxs, out_shifts, out_negs, ops_i, ops_f);
+    });
+}
+
+void da4ml_split_free(da4ml_split_t *s) { delete s; }
 
 void da4ml_pipeline_free(da4ml_pipeline_t *p) { delete p; }
 int64_t da4ml_pipeline_n_stages(const da4ml_pipeline_t *p) { return p ? (int64_t)p->impl->stages.size() : 0; }

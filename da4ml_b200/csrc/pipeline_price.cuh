@@ -100,6 +100,36 @@ DA_HD double pp_bitsd(unsigned long long u) {
     return x;
 }
 
+// The tracer's latency of every adder node of task `t`, level by level, with the tracer's own expressions (t.lat holds the
+// inputs' latencies on entry); the first failing adder goes to `s_fail` as (node << 2 | status).  With COST, cost_add's
+// cost of every adder node goes to cost[node] as well (the split needs it, pricing drops it).  Every thread of the CTA
+// calls it; it ends with a barrier.  Shared by pipeline_price_kernel and pipeline_split_kernel.
+template <bool COST> __device__ __forceinline__ void pp_replay(const PpDesign &d, const PpTask &t, unsigned long long &s_fail, float *cost_out) {
+    const double c = t.cutoff;
+    const int tid = threadIdx.x, nt = blockDim.x;
+    for (int l = 0; l < d.n_levels; ++l) {
+        for (int k = d.lvl_begin[l] + tid; k < d.lvl_begin[l + 1]; k += nt) {
+            const PpAdd a = d.adds[k];
+            float dl = 0.f, cost = 0.f;
+            cost_add(QInt{a.q0[0], a.q0[1], a.q0[2]}, QInt{a.q1[0], a.q1[1], a.q1[2]}, 0, false, d.adder_size, d.carry_size, dl, cost);
+            const double dlat = (double)dl, base = fmax(t.lat[a.n0], t.lat[a.n1]);
+            double lat = pp_add(dlat, base);
+            bool slow = false;
+            if (c > 0 && ceil(pp_div(lat, c)) > ceil(pp_div(base, c))) { // would straddle a register boundary
+                slow = !(dlat <= c);
+                lat = pp_add(pp_mul(ceil(pp_div(base, c)), c), dlat);
+            }
+            t.lat[a.node] = lat;
+            if (COST)
+                cost_out[a.node] = cost;
+            const int st = a.flag == 2 ? PP_UNSUPPORTED : slow ? PP_SLOW_ADDER : a.flag == 1 ? PP_UNSUPPORTED : PP_OK;
+            if (st != PP_OK)
+                atomicMin(&s_fail, ((unsigned long long)a.node << 2) | (unsigned long long)st);
+        }
+        __syncthreads();
+    }
+}
+
 __global__ void __launch_bounds__(256) pipeline_price_kernel(const PpDesign *designs, const PpTask *tasks, PpResult *results) {
     DA_SHARED_VAR(unsigned long long, s_fail);  // (replay order << 2 | status) of the first failing adder
     DA_SHARED_VAR(unsigned long long, s_latmax);
@@ -121,25 +151,7 @@ __global__ void __launch_bounds__(256) pipeline_price_kernel(const PpDesign *des
         t.last_use[v] = -1;
     }
     __syncthreads();
-    for (int l = 0; l < d.n_levels; ++l) {
-        for (int k = d.lvl_begin[l] + tid; k < d.lvl_begin[l + 1]; k += nt) {
-            const PpAdd a = d.adds[k];
-            float dl = 0.f, cost = 0.f;
-            cost_add(QInt{a.q0[0], a.q0[1], a.q0[2]}, QInt{a.q1[0], a.q1[1], a.q1[2]}, 0, false, d.adder_size, d.carry_size, dl, cost);
-            const double dlat = (double)dl, base = fmax(t.lat[a.n0], t.lat[a.n1]);
-            double lat = pp_add(dlat, base);
-            bool slow = false;
-            if (c > 0 && ceil(pp_div(lat, c)) > ceil(pp_div(base, c))) { // would straddle a register boundary
-                slow = !(dlat <= c);
-                lat = pp_add(pp_mul(ceil(pp_div(base, c)), c), dlat);
-            }
-            t.lat[a.node] = lat;
-            const int st = a.flag == 2 ? PP_UNSUPPORTED : slow ? PP_SLOW_ADDER : a.flag == 1 ? PP_UNSUPPORTED : PP_OK;
-            if (st != PP_OK)
-                atomicMin(&s_fail, ((unsigned long long)a.node << 2) | (unsigned long long)st);
-        }
-        __syncthreads();
-    }
+    pp_replay<false>(d, t, s_fail, nullptr);
     PpResult r{};
     if (s_fail != ~0ull) {
         if (tid == 0) {
@@ -218,6 +230,17 @@ struct PpStageIn {
     const float *ops_f;                                                     // [n_ops][5]
 };
 
+// What a split needs beyond pricing, recorded by pp_prepare only when asked for (pipeline_split.cuh).  Node ids as in
+// PpDesign; the constant node stands for every all-zero output column.
+struct PpSplitInfo {
+    std::vector<double> own_q;          // [n_nodes][3] the node's own (unscaled) interval; the constant: (0, 0, 2^32)
+    std::vector<int> x, y, opc, data;   // per adder node - n_in - 1: FixedVariable.__add__'s operand order (the operand
+                                        // with a positive factor first) and the op it becomes: opcode = (factor of y < 0),
+                                        // data = log2|factor of y / factor of x|
+    std::vector<int64_t> out_shift;     // [n_out] log2|factor| of each output's view
+    std::vector<char> out_neg;          // [n_out] factor < 0
+};
+
 struct PpPrepared {
     std::vector<PpAdd> adds;
     std::vector<int> lvl_begin, node_bits, out_node;
@@ -237,7 +260,7 @@ inline int pp_kif_bits(double lo, double hi, double step) {
 }
 
 // Check one design's arrays (DA4ML_E_INVALID-class errors are thrown as std::invalid_argument) and prepare it.
-inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages) {
+inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo *split = nullptr) {
     struct View { // a node seen through a scaling: interval of the scaled value and its factor (+-2^k)
         int node;
         double lo, hi, step, f;
@@ -322,6 +345,12 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages) {
             }
             a.q0[0] = (float)X.lo, a.q0[1] = (float)X.hi, a.q0[2] = (float)X.step;
             a.q1[0] = (float)Y.lo, a.q1[1] = (float)Y.hi, a.q1[2] = (float)Y.step;
+            if (split) {
+                split->x.push_back(X.node);
+                split->y.push_back(Y.node);
+                split->opc.push_back(Y.f < 0);
+                split->data.push_back((int)std::log2(std::fabs(Y.f / X.f)));
+            }
             if (a.flag == 0 && lo == hi)
                 a.flag = 1;
             node_view.push_back(View{a.node, lo, hi, step, f});
@@ -341,6 +370,18 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages) {
     }
     P.n_nodes = P.n_in + 1 + (int)adds.size();
     P.n_out = (int)cur.size();
+    if (split) {
+        split->own_q.resize(3 * (size_t)P.n_nodes);
+        for (int v = 0; v < P.n_nodes; ++v) {
+            View w = view_of(v);
+            w = scaled(w, 1.0 / w.f); // FixedVariable.unscaled
+            split->own_q[3 * v] = w.lo, split->own_q[3 * v + 1] = w.hi, split->own_q[3 * v + 2] = w.step;
+        }
+        for (const View &v : cur) {
+            split->out_shift.push_back((int64_t)std::log2(std::fabs(v.f)));
+            split->out_neg.push_back(v.f < 0);
+        }
+    }
     // liveness (comb_trace's dead-statement elimination) and bits
     std::vector<char> live(P.n_nodes, 0);
     for (const View &v : cur) {
@@ -385,6 +426,8 @@ struct PpAnswer {
     int status = PP_OK, stages = -1;
     long long reg_bits = -1;
     double latency_max = 0, cutoff = 0;
+    int first_stages = -1; // stages of the first split (the task's own cutoff and latencies)
+    bool retimed = false;  // a bisection round succeeded: the kept split is the last such round's (`cutoff`, latency 0)
 };
 
 // `run(tasks, results)`: one launch of pipeline_price_kernel over `tasks` (design, cutoff, latencies: nullptr = zeros).
@@ -417,7 +460,7 @@ inline std::vector<PpAnswer> pp_price(int n_designs, const double *cutoffs, int 
     }
     std::vector<int> n_stages(req.size());
     for (size_t t = 0; t < req.size(); ++t)
-        n_stages[t] = ans[t].stages;
+        n_stages[t] = ans[t].first_stages = ans[t].stages;
     while (retiming) {
         std::vector<size_t> open;
         std::vector<PpRequest> round;
@@ -436,6 +479,7 @@ inline std::vector<PpAnswer> pp_price(int n_designs, const double *cutoffs, int 
                 continue;
             }
             hi[t] = round[k].cutoff;
+            ans[t].retimed = true;
             ans[t].stages = res[k].stages;
             ans[t].reg_bits = res[k].reg_bits;
         }

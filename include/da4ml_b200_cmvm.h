@@ -238,6 +238,33 @@ int da4ml_pipeline_price(
     double *out_latency, double profile[2]
 );
 
+/* Pipelined pricing that also builds and keeps the register stages (the split) of every ok task on the GPU: the
+ * arguments and outputs of da4ml_pipeline_price, profile (NULL to skip) = {device_ms, launches, split launches, bytes of
+ * op tables copied back}, and *out a handle to free with da4ml_split_free.  The split of task (d, j) is what the
+ * reference's to_pipeline(comb, c, retiming) returns: without retiming, the split of the trace under d's input latencies;
+ * with it, retime_pipeline's (the first split when no bisection round succeeded, else the last successful round's, at
+ * cutoff_out with every input at latency 0).  Arguments are checked on the host before any device call. */
+typedef struct da4ml_split da4ml_split_t; /* opaque split result */
+int da4ml_pipeline_split(
+    int64_t n_designs, const int64_t *n_stages, const int64_t *stage_meta, const int64_t *inp_shifts,
+    const int64_t *out_idxs, const int64_t *out_shifts, const int64_t *out_negs, const int64_t *ops_i,
+    const float *ops_f, const double *latencies, const double *cutoffs, int64_t n_cutoffs, int retiming,
+    int32_t *status, int64_t *stages, int64_t *reg_bits, double *latency_max, double *cutoff_out,
+    double *out_latency, double profile[4], da4ml_split_t **out
+);
+/* task = d * n_cutoffs + j: out = {status, n_stages, n_rows, n_outs}; status 0: split kept, 1: the task is not ok (no
+ * split), 2: the reference's to_pipeline raises KeyError on the task (a stage would have no op or no output, as when
+ * every input arrives after the first stage). */
+int da4ml_split_info(const da4ml_split_t *s, int64_t task, int64_t out[4]);
+/* A kept split's stages, concatenated in stage order: stage_meta [n_stages][3] = {n_in, n_out, n_ops}; out_idxs,
+ * out_shifts, out_negs [n_outs] (shifts and negations are the design's in the last stage, 0 before); ops_i [n_rows][4];
+ * ops_f [n_rows][5] in float64 (copy latencies c * (j + 1) and traced latencies are doubles).  inp_shifts are all 0. */
+int da4ml_split_copy(const da4ml_split_t *s, int64_t task, int64_t *stage_meta, int64_t *out_idxs, int64_t *out_shifts,
+                     int64_t *out_negs, int64_t *ops_i, double *ops_f);
+/* Both accessors give DA4ML_E_INVALID, with the reason in da4ml_cmvm_last_error, for a null handle or array, a task out
+ * of range, or (da4ml_split_copy) a task without a split. */
+void da4ml_split_free(da4ml_split_t *s);
+
 /* ---- DAIS interpreter (SURVEY 8f N2) ----------------------------------------------------------------
  * Replaces `run_interp` of the reference's second native module (dais/bindings.cc:30-131 -> DAISInterpreter.cc) for
  * every DAIS program: all opcodes of DAISInterpreter::exec_ops and lookup tables.  Programs are the int32 words of
