@@ -742,6 +742,11 @@ class ChainFront(NetworkFront):
         """Point ``p``'s designs as one ``Pipeline`` per layer."""
         return [r.to_pipeline(types_module) for r in self._raws[p]]
 
+    def design(self, p: int, activations) -> RawPipeline:
+        """Point ``p``'s designs as one chain design with ``activations`` between the layers: ``chain_design(self.pipelines(p),
+        activations)``, for ``price_pipelined`` (register bits, ``keep_split``)."""
+        return chain_design(self._raws[p], activations)
+
     def reference_calls(self, p: int) -> list[dict]:
         """Per layer, the keywords of the ``solve(kernels[k], **kw)`` call that returns layer ``k``'s design in point
         ``p``: the candidate's options, the layer's ``qintervals`` and its input ``latencies`` as Python floats (for
@@ -817,8 +822,9 @@ def chain_front(kernels, option_sets, qintervals=None, latencies=None, adder_siz
     candidate whose status is not ok (an adder slower than ``c``) is dropped (``profile['layers'][k]['dropped']``).
     ``stages[p] = floor(latency / (c + 1e-9)) + 1`` is the clock count ``to_pipeline`` gives the chain when its network
     inputs arrive before ``c``; ``retime_pipeline`` never accepts a split with more stages, so retiming never adds a
-    clock.  ``best_stages(n)`` is the cheapest point with at most ``n`` stages.  Register bits of a whole chain are not
-    reported: the activation ops between layers have widths of their own, so they are not the sum of the layers'.
+    clock.  ``best_stages(n)`` is the cheapest point with at most ``n`` stages.  A point's register bits and register
+    stages as one pipeline, with the activations between its layers, are ``price_pipelined(front.design(p,
+    activations), c, keep_split=True)`` (``chain_design``).
     Activations between layers add no latency, as ``relu`` and ``wrap`` in the tracer keep their input's latency.  The
     front is the front of the chains explored: the solver is not monotone in its input latencies, so pruning partial
     chains on (cost, latency) is a heuristic and a pruned chain could have led to a better design.  What is reported is
@@ -875,6 +881,177 @@ def chain_front(kernels, option_sets, qintervals=None, latencies=None, adder_siz
     cost, lat, choice, _, raws, calls = points
     order = np.argsort(lat, kind='stable')
     return ChainFront(cost[order], lat[order], choice[order], [raws[p] for p in order], [calls[p] for p in order], prof, c)
+
+
+def _kif_prop(lo: float, hi: float, step: float) -> tuple[int, int, int]:
+    """``FixedVariable.kif`` (reference trace/fixed_variable.py:418-428) of a non-constant value."""
+    return int(lo < 0), int(np.ceil(np.log2(max(-lo, hi + step)))), -int(np.log2(step))
+
+
+def _activate(kind: str, lo: float, hi: float, step: float, k: int, i: int, f: int):
+    """What the tracer's ``relu(i, f)`` (TRN, trace/fixed_variable.py:645-686) or ``quantize(k, i, f)`` (WRAP / TRN,
+    :688-779) makes of a non-constant value [lo, hi] / step: ``None`` (the value itself), or the (lo, hi, step) of the result
+    (lo == hi: a constant).  Every number is a dyadic rational, exact in float64."""
+    from math import ceil, floor
+
+    if kind == 'relu':
+        st = max(2.0**-f, step)
+        l, h = floor(max(0.0, lo) / st) * st, floor(hi / st) * st
+        if 2.0**i - st < h:
+            l, h = 0.0, 2.0**i - st
+        h = max(0.0, h)
+        return None if (l, h, st) == (lo, hi, step) else (l, h, st)
+    if k + i + f <= 0:
+        return 0.0, 0.0, 1.0
+    k0, i0, f0 = _kif_prop(lo, hi, step)
+    if k >= k0 and i >= i0 and f >= f0:
+        return None
+    f = min(f, f0)
+    k = min(k, k0) if i >= i0 else k
+    st = 2.0**-f
+    if lo < 0:
+        i0 = max(i0, ceil(np.log2(-(floor(lo / st) * st))))
+    i = min(i, i0 + int(k == 0 and k0 == 1))
+    if i + k + f <= 0:
+        return 0.0, 0.0, 1.0
+    l, h = -k * 2.0**i, 2.0**i - st
+    if lo >= l and hi <= h:
+        l, h = floor(lo / st) * st, floor(hi / st) * st
+    return l, h, st
+
+
+def _traced_intervals(stages, vals):
+    """The intervals (lo, hi, step) of a design's outputs as the tracer's replay (``CombLogic.__call__`` on
+    ``FixedVariable``s) gives them for inputs of intervals ``vals``: sums of the operands' scaled intervals, which can be
+    wider than the ones the solver records.  A dead column is the constant 0, (0, 0, 1)."""
+    for st in stages:
+        ins = [(lo * 2.0**sh, hi * 2.0**sh, s * 2.0**sh) for (lo, hi, s), sh in zip(vals, np.asarray(st['inp_shifts'], np.int64).tolist())]
+        buf = []
+        for id0, id1, opc, data in np.asarray(st['ops_i'], np.int64).reshape(-1, 4).tolist():
+            if opc == -1:
+                buf.append(ins[id0])
+                continue
+            a, (lo, hi, s) = buf[id0], buf[id1]
+            b = (lo * 2.0**data, hi * 2.0**data, s * 2.0**data)
+            if opc == 1:
+                b = (-b[1], -b[0], b[2])
+            buf.append((a[0] + b[0], a[1] + b[1], min(a[2], b[2])) if a[0] != a[1] and b[0] != b[1] else (b if a[0] == a[1] else a))
+        vals = []
+        for i, sh, ng in zip(np.asarray(st['out_idxs'], np.int64).tolist(), np.asarray(st['out_shifts'], np.int64).tolist(), np.asarray(st['out_negs']).astype(bool).tolist()):
+            if i < 0:
+                vals.append((0.0, 0.0, 1.0))
+                continue
+            lo, hi, s = (v * 2.0**sh for v in buf[i])
+            vals.append((-hi, -lo, s) if ng else (lo, hi, s))
+    return vals
+
+
+def _act_arg(k: int, act, n: int):
+    """(kind, [n, 3] int64 kif) of activation ``k`` of ``chain_design``."""
+    if not isinstance(act, (tuple, list)) or len(act) not in (2, 3, 4):
+        raise ValueError(f"activation {k}: expected ('quantize' | 'relu', kif[, round_mode[, overflow_mode]]), got {act!r}")
+    kind, kif, *modes = act
+    if kind not in ('quantize', 'relu'):
+        raise ValueError(f"activation {k}: {kind!r} is not 'quantize' or 'relu'")
+    if len(modes) > 0 and str(modes[0]).upper() != 'TRN':
+        raise ValueError(f'activation {k}: rounding mode {modes[0]!r} is not covered (only TRN)')
+    if len(modes) > 1 and str(modes[1]).upper() != 'WRAP':
+        raise ValueError(f'activation {k}: overflow mode {modes[1]!r} is not covered (only WRAP)')
+    a = np.asarray(kif)
+    if a.dtype == bool:
+        a = a.astype(np.int64)
+    if a.size == 0 or not (np.issubdtype(a.dtype, np.integer) or (np.issubdtype(a.dtype, np.floating) and np.all(np.isfinite(a)) and np.all(a == np.round(a)))):
+        raise ValueError(f'activation {k}: kif must be integers')
+    a = a.astype(np.int64)
+    if a.shape == (3,):
+        a = np.tile(a, (n, 1))
+    if a.shape != (n, 3):
+        raise ValueError(f'activation {k}: kif must be one (k, i, f) triple or [{n}, 3], got shape {np.asarray(kif).shape}')
+    if not np.isin(a[:, 0], (0, 1)).all() or (kind == 'relu' and (a[:, 0] != 0).any()):
+        raise ValueError(f"activation {k}: k must be 0 or 1" + (" (0 for 'relu': its output is unsigned)" if kind == 'relu' else ''))
+    if (np.abs(a[:, 1:]) > 64).any():
+        raise ValueError(f'activation {k}: i and f must be within [-64, 64]')
+    return kind, a
+
+
+def chain_design(designs, activations) -> RawPipeline:
+    """A chain of solver designs with a relu or quantizer between consecutive layers, as ONE design: layer 0's stages, an
+    activation stage, layer 1's stages, and so on.  ``price_pipelined`` prices and splits it as the reference's tracer
+    pipelines the whole model: ``to_pipeline(comb_trace(inp, chain(inp)), c, retiming)``, where ``chain`` replays every
+    layer with ``CombLogic.__call__`` and applies ``relu`` / ``quantize`` between them; its register stages can fall inside
+    and across layers.
+
+    ``designs``: solver results (``RawPipeline``, stage-dict lists or ``Pipeline`` containers), layer ``k``'s output count
+    equal to layer ``k + 1``'s input count, all with the same ``adder_size`` / ``carry_size``.  ``activations[k]`` is the
+    op between layer ``k`` and layer ``k + 1``: ``('relu', kif)`` for ``relu(i, f)`` or ``('quantize', kif)`` for
+    ``quantize(k, i, f)``, with ``kif`` one ``(k, i, f)`` triple for every output or an ``[n_out_k, 3]`` int array (``k``
+    is 0 for relu).  Rounding is TRN and overflow WRAP; an optional third and fourth element may name them, and any other
+    mode is a ``ValueError``.
+
+    An activation stage has one input op per value (opcode -1, the value's interval ``Pipeline.out_qint`` and latency), and
+    one op per value the activation changes, with the fields the tracer records for it: opcode 2 (relu) or 3 (quantize)
+    reading that input, data 0, the result's interval and the tracer's cost (``sum(kif) / 2`` for relu, 0 for quantize).
+    Intervals are the ones the tracer's replay of the layers gives, which can be wider than the solver's.  Latencies are
+    the value's as its layer's design records it (relu and quantize add none); a layer's design is solved as if its
+    inputs arrived at 0, and ``price_pipelined`` re-traces every latency anyway.  A value the tracer passes through unchanged (``quantize`` to a
+    wider format, ``relu`` of a non-negative value) gets no op: its output reads the input op.  A value that becomes the
+    constant 0 (a dead column, or a format with no bits left) is a dead output column (``out_idx -1``).  A value that would
+    become any other constant is refused with ``ValueError``.  All checks run on the host, before any device call."""
+    stages = [_design_stages(d) for d in designs]
+    if not stages:
+        raise ValueError('chain_design needs at least one design')
+    acts = list(activations)
+    if len(acts) != len(stages) - 1:
+        raise ValueError(f'{len(stages)} designs need {len(stages) - 1} activations, got {len(acts)}')
+    sizes = {(int(d[0]['adder_size']), int(d[0]['carry_size'])) for d in stages}
+    if len(sizes) != 1:
+        raise ValueError(f'the designs of a chain must share adder_size and carry_size, got {sorted(sizes)}')
+    a_sz, c_sz = sizes.pop()
+    for k in range(1, len(stages)):
+        if stages[k - 1][-1]['shape'][1] != stages[k][0]['shape'][0]:
+            raise ValueError(f"layer {k - 1} has {stages[k - 1][-1]['shape'][1]} outputs but layer {k} has {stages[k][0]['shape'][0]} inputs")
+    kinds = [_act_arg(k, act, int(stages[k][-1]['shape'][1])) for k, act in enumerate(acts)]
+    s0 = stages[0][0]
+    vals = [(0.0, 0.0, 1.0)] * int(s0['shape'][0])  # (CombLogic.inp_qint)
+    for (id0, _, opc, _), q in zip(np.asarray(s0['ops_i'], np.int64).reshape(-1, 4).tolist(), np.asarray(s0['ops_f'], np.float64).reshape(-1, 5).tolist()):
+        if opc == -1:
+            vals[id0] = tuple(q[:3])
+    out = [dict(st) for st in stages[0]]
+    for k, (kind, kif) in enumerate(kinds):
+        last = stages[k][-1]
+        n = int(last['shape'][1])
+        vals = _traced_intervals(stages[k], vals)
+        idx = np.asarray(last['out_idxs'], np.int64)
+        of = np.asarray(last['ops_f'], np.float64).reshape(-1, 5)
+        ops_i, ops_f, out_idxs = [], [], np.zeros(n, np.int64)
+        for j in range(n):  # the input ops first, in value order: the traced interval and the solver's latency
+            ops_i.append([j, -1, -1, 0])
+            ops_f.append([*vals[j], float(of[idx[j], 3]) if idx[j] >= 0 else 0.0, 0.0])
+        for j in range(n):
+            lo, hi, st, lat = ops_f[j][0], ops_f[j][1], ops_f[j][2], ops_f[j][3]
+            if idx[j] < 0 or lo == hi:
+                if lo != 0.0 or hi != 0.0:
+                    raise ValueError(f'activation {k}: output {j} of layer {k} is the constant {lo} (only the constant 0 is covered)')
+                out_idxs[j] = -1
+                continue
+            r = _activate(kind, lo, hi, st, *(int(v) for v in kif[j]))
+            if r is None:
+                out_idxs[j] = j
+                continue
+            if r[0] == r[1]:
+                if r[0] != 0.0:
+                    raise ValueError(f'activation {k}: output {j} becomes the constant {r[0]} (only the constant 0 is covered)')
+                out_idxs[j] = -1
+                continue
+            cost = sum(_kif_prop(*r)) / 2 if kind == 'relu' else 0.0
+            out_idxs[j] = len(ops_i)
+            ops_i.append([j, -1, 2 if kind == 'relu' else 3, 0])
+            ops_f.append([*r, lat, cost])
+        vals = [tuple(ops_f[i][:3]) if i >= 0 else (0.0, 0.0, 1.0) for i in out_idxs.tolist()]
+        out.append(dict(shape=(n, n), inp_shifts=np.zeros(n, np.int64), out_idxs=out_idxs, out_shifts=np.zeros(n, np.int64), out_negs=np.zeros(n, np.int64),
+                        ops_i=np.asarray(ops_i, np.int64).reshape(-1, 4), ops_f=np.asarray(ops_f, np.float32).reshape(-1, 5), adder_size=a_sz, carry_size=c_sz))
+        out += [dict(st) for st in stages[k + 1]]
+    return RawPipeline.from_stages(out)
 
 
 PRICE_STATUS = ['ok', 'adder slower than the cutoff', 'not supported']  # PipelinePrice.status codes 0, 1, 2

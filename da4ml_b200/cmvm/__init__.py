@@ -7,11 +7,12 @@ chain of layers under a latency budget, and ``chain_front`` for the same with ea
 of the design before it (the designs and latencies a traced model gets).  ``solve``'s ``seed`` keyword picks the
 tie-break order of the greedy pair selection (0 = the reference's), and ``solve_best_of`` keeps the cheapest of many seeds.
 ``price_pipelined`` prices designs as they will be pipelined under a latency cutoff: clock stages, register bits and the
-tracer's latencies."""
+tracer's latencies; ``chain_design`` joins a chain's designs, with the relu / quantizers between its layers, into one
+design that it prices and splits as one pipeline."""
 
 from typing import TypedDict
 
-from .._binary import (ChainFront, NetworkFront, PipelinePrice, SweepResult, chain_front, kernel_decompose, network_front, price_pipelined, solve, solve_batch,
+from .._binary import (ChainFront, NetworkFront, PipelinePrice, SweepResult, chain_design, chain_front, kernel_decompose, network_front, price_pipelined, solve, solve_batch,
                        solve_best_of, solve_sweep, solve_sweep_batch)  # fmt: skip
 from ..batching import CmvmCall, SolveBatcher, solve_calls
 from ..types import CombLogic, Op, Pipeline, QInterval
@@ -34,4 +35,4 @@ solver_options_t = TypedDict(
     total=False,
 )
 
-__all__ = ['solve', 'solve_batch', 'solve_best_of', 'solve_sweep', 'solve_sweep_batch', 'SweepResult', 'network_front', 'NetworkFront', 'chain_front', 'ChainFront', 'price_pipelined', 'PipelinePrice', 'solve_calls', 'CmvmCall', 'SolveBatcher', 'kernel_decompose', 'QInterval', 'Op', 'CombLogic', 'Pipeline', 'solver_options_t']
+__all__ = ['solve', 'solve_batch', 'solve_best_of', 'solve_sweep', 'solve_sweep_batch', 'SweepResult', 'network_front', 'NetworkFront', 'chain_front', 'ChainFront', 'chain_design', 'price_pipelined', 'PipelinePrice', 'solve_calls', 'CmvmCall', 'SolveBatcher', 'kernel_decompose', 'QInterval', 'Op', 'CombLogic', 'Pipeline', 'solver_options_t']

@@ -30,7 +30,9 @@ enum PpStatus : int { PP_OK = 0, PP_SLOW_ADDER = 1 /* the tracer's AssertionErro
 
 // One adder of a design, in dependency-level order.  `node` is its own node id; n0 / n1 the nodes its operands view; q0 /
 // q1 the operand intervals cost_add receives (after FixedVariable.__add__'s sign normalisation, as float32); `flag` 2: an
-// operand is a constant (refused before the latency), 1: the sum is a constant (refused after the latency), 0: neither.
+// operand is a constant (refused before the latency), 1: the sum is a constant (refused after the latency), 0: neither;
+// 3: not an adder but an activation (relu / quantize, opcodes +-2 / +-3) of node n0 == n1, which keeps its operand's
+// latency (trace/fixed_variable.py:381-384) and whose tracer cost is q0[0].
 struct PpAdd {
     int node, n0, n1, flag;
     float q0[3], q1[3];
@@ -110,6 +112,12 @@ template <bool COST> __device__ __forceinline__ void pp_replay(const PpDesign &d
     for (int l = 0; l < d.n_levels; ++l) {
         for (int k = d.lvl_begin[l] + tid; k < d.lvl_begin[l + 1]; k += nt) {
             const PpAdd a = d.adds[k];
+            if (a.flag == 3) { // an activation (relu / quantize): its operand's latency, no adder
+                t.lat[a.node] = t.lat[a.n0];
+                if (COST)
+                    cost_out[a.node] = a.q0[0];
+                continue;
+            }
             float dl = 0.f, cost = 0.f;
             cost_add(QInt{a.q0[0], a.q0[1], a.q0[2]}, QInt{a.q1[0], a.q1[1], a.q1[2]}, 0, false, d.adder_size, d.carry_size, dl, cost);
             const double dlat = (double)dl, base = fmax(t.lat[a.n0], t.lat[a.n1]);
@@ -236,7 +244,11 @@ struct PpSplitInfo {
     std::vector<double> own_q;          // [n_nodes][3] the node's own (unscaled) interval; the constant: (0, 0, 2^32)
     std::vector<int> x, y, opc, data;   // per adder node - n_in - 1: FixedVariable.__add__'s operand order (the operand
                                         // with a positive factor first) and the op it becomes: opcode = (factor of y < 0),
-                                        // data = log2|factor of y / factor of x|
+                                        // data = log2|factor of y / factor of x|; an activation: x its operand, y -1,
+                                        // opcode +-2 / +-3 by the sign of the operand's factor, data 0
+    std::vector<double> xv, yv;         // per adder node - n_in - 1: the views x and y themselves, (lo, hi, step, factor)
+                                        // (y: zeros for an activation)
+    std::vector<double> out_v;          // [n_out][4] each output's view
     std::vector<int64_t> out_shift;     // [n_out] log2|factor| of each output's view
     std::vector<char> out_neg;          // [n_out] factor < 0
 };
@@ -247,6 +259,62 @@ struct PpPrepared {
     int n_in = 0, n_nodes = 0, n_out = 0, adder_size = -1, carry_size = -1;
     long long out_bits = 0;
 };
+
+// minimal_kif (types.py:86-114) of an interval
+inline void pp_minimal_kif(double lo, double hi, double step, int &k, int &i, int &f) {
+    if (lo == 0.0 && hi == 0.0) {
+        k = i = f = 0;
+        return;
+    }
+    k = lo < 0;
+    f = (int)(-std::log2(step));
+    const double imin = std::nearbyint(lo / step), imax = std::nearbyint(hi / step);
+    i = (int)std::ceil(std::log2(std::max(std::fabs(imin), imax + 1))) - f;
+}
+
+// What relu / quantize make of a value (the interval [lo, hi] of its scaled view, step > 0), as CombLogic.__call__ replays
+// opcodes +-2 / +-3 (types.py:259-266): FixedVariable.relu(i, f) with TRN (trace/fixed_variable.py:645-686) and
+// FixedVariable.quantize(k, i, f) with WRAP / TRN and _force_factor_clear (:688-779), (k, i, f) the minimal_kif of the op's
+// interval.  kind 0: the value itself (relu changed nothing), 1: the constant `lo`, 2: a new value [lo, hi] / step.
+struct PpAct {
+    int kind;
+    double lo, hi, step;
+};
+// FixedVariable.kif (trace/fixed_variable.py:418-428) of a non-constant value: k + i + f
+inline int pp_kif_prop_bits(double lo, double hi, double step) {
+    const int f = -(int)std::log2(step);
+    const int i = (int)std::ceil(std::log2(std::max(-lo, hi + step)));
+    return (lo < 0) + i + f;
+}
+inline PpAct pp_relu(double lo, double hi, double step, int i, int f) {
+    const double st = std::max(std::ldexp(1.0, -f), step);
+    double l = (std::floor(std::max(0.0, lo) / st) + 0.0) * st, h = (std::floor(hi / st) + 0.0) * st; // (floor: an int, no -0)
+    const double top = std::ldexp(1.0, i) - st;
+    if (top < h)
+        l = 0.0, h = top;
+    h = std::max(0.0, h);
+    if (l == lo && h == hi && st == step)
+        return PpAct{0, lo, hi, step};
+    return l == h ? PpAct{1, l, l, st} : PpAct{2, l, h, st};
+}
+inline PpAct pp_quantize(double lo, double hi, double step, int k, int i, int f) {
+    if (k + i + f <= 0)
+        return PpAct{1, 0.0, 0.0, 1.0};
+    const int f0 = -(int)std::log2(step), k0 = lo < 0;
+    int i0 = (int)std::ceil(std::log2(std::max(-lo, hi + step)));
+    f = std::min(f, f0);
+    k = i >= i0 ? std::min(k, k0) : k;
+    const double st = std::ldexp(1.0, -f);
+    if (lo < 0)
+        i0 = std::max(i0, (int)std::ceil(std::log2(-std::floor(lo / st) * st)));
+    i = std::min(i, i0 + (k == 0 && k0 == 1));
+    if (i + k + f <= 0)
+        return PpAct{1, 0.0, 0.0, 1.0};
+    double l = k ? -std::ldexp(1.0, i) : 0.0, h = std::ldexp(1.0, i) - st; // (+0.0, as the tracer's Decimal)
+    if (lo >= l && hi <= h)
+        l = (std::floor(lo / st) + 0.0) * st, h = (std::floor(hi / st) + 0.0) * st;
+    return l == h ? PpAct{1, l, l, st} : PpAct{2, l, h, st};
+}
 
 // sum of minimal_kif (types.py:86-114) of an interval
 inline int pp_kif_bits(double lo, double hi, double step) {
@@ -269,6 +337,8 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
         const double a = v.lo * s, b = v.hi * s;
         return View{v.node, std::min(a, b), std::max(a, b), std::fabs(v.step * s), v.f * s};
     };
+    // FixedVariable.__neg__: Decimal negation, whose zero is +0 (a product with a negative power of two gives -0)
+    auto negated = [](View v) { return View{v.node, 0.0 - v.hi, 0.0 - v.lo, v.step, -v.f}; };
     auto bad = [](const std::string &m) { throw std::invalid_argument("pipeline_price: " + m); };
     if (n_stages < 1)
         bad("a design needs at least one stage");
@@ -291,10 +361,24 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
             bad("a stage array is null");
         for (int64_t i = 0; i < S.n_ops; ++i) {
             const int64_t *o = S.ops_i + 4 * i;
-            const bool ok = o[2] == -1 ? (o[0] >= 0 && o[0] < S.n_in && std::abs(S.inp_shifts[o[0]]) <= 512) : (o[2] == 0 || o[2] == 1) ? (o[0] >= 0 && o[0] < i && o[1] >= 0 && o[1] < i && std::abs(o[3]) <= 512) : false;
+            const bool act = o[2] == 2 || o[2] == -2 || o[2] == 3 || o[2] == -3;
+            const bool ok = o[2] == -1 ? (o[0] >= 0 && o[0] < S.n_in && std::abs(S.inp_shifts[o[0]]) <= 512)
+                            : (o[2] == 0 || o[2] == 1) ? (o[0] >= 0 && o[0] < i && o[1] >= 0 && o[1] < i && std::abs(o[3]) <= 512)
+                            : act ? (o[0] >= 0 && o[0] < i && o[1] == -1 && o[3] == 0)
+                                  : false;
             if (!ok)
                 bad("stage " + std::to_string(s) + " op " + std::to_string(i) + ": opcode " + std::to_string(o[2]) + " with operands (" + std::to_string(o[0]) + ", " +
-                    std::to_string(o[1]) + ") is not an adder-graph op (opcodes -1, 0, 1; operands earlier ops, inputs in range)");
+                    std::to_string(o[1]) + ") is not an adder-graph op (opcodes -1, 0, 1 and the activations +-2, +-3; operands earlier ops, inputs in range)");
+            if (act) { // the op's interval gives the activation's (k, i, f): a finite interval on a power-of-two grid
+                const float *q = S.ops_f + 5 * i;
+                const double lo = q[0], hi = q[1], st = q[2];
+                int e = 0;
+                const bool grid = std::isfinite(lo) && std::isfinite(hi) && st > 0 && std::isfinite(st) && std::frexp(st, &e) == 0.5 && lo <= hi &&
+                                  std::fabs(lo / st) < 9.0e15 && std::fabs(hi / st) < 9.0e15 && lo / st == std::trunc(lo / st) && hi / st == std::trunc(hi / st);
+                if (!grid)
+                    bad("stage " + std::to_string(s) + " op " + std::to_string(i) + ": the interval of an activation is not a quantized interval (min <= max, "
+                        "multiples of a power-of-two step)");
+            }
         }
         for (int64_t k = 0; k < S.n_out; ++k)
             if (S.out_idxs[k] < -1 || S.out_idxs[k] >= S.n_ops || std::abs(S.out_shifts[k]) > 512)
@@ -326,26 +410,76 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
                 buf[i] = scaled(cur[o[0]], std::ldexp(1.0, (int)S.inp_shifts[o[0]]));
                 continue;
             }
+            if (o[2] != 0 && o[2] != 1) { // relu (+-2) / quantize (+-3) of the operand (negated for the negative opcode)
+                View V = o[2] < 0 ? negated(buf[o[0]]) : buf[o[0]];
+                if (V.lo == V.hi) { // a constant: the tracer folds it (relu / quantize of 0 is 0)
+                    if (V.lo != 0.0)
+                        bad("stage " + std::to_string(s) + " op " + std::to_string(i) + ": an activation of the constant " + std::to_string(V.lo) +
+                            " (only the constant 0 is covered)");
+                    buf[i] = view_of(CONST);
+                    continue;
+                }
+                const float *q = S.ops_f + 5 * i;
+                int kk, ii, ff;
+                pp_minimal_kif(q[0], q[1], q[2], kk, ii, ff);
+                const bool relu = std::abs(o[2]) == 2;
+                const PpAct r = relu ? pp_relu(V.lo, V.hi, V.step, ii, ff) : pp_quantize(V.lo, V.hi, V.step, kk, ii, ff);
+                if (r.kind == 0) {
+                    buf[i] = V;
+                    continue;
+                }
+                if (r.kind == 1) {
+                    if (r.lo != 0.0)
+                        bad("stage " + std::to_string(s) + " op " + std::to_string(i) + ": the activation makes the constant " + std::to_string(r.lo) +
+                            " (only the constant 0 is covered)");
+                    buf[i] = view_of(CONST);
+                    continue;
+                }
+                PpAdd a{};
+                a.node = P.n_in + 1 + (int)adds.size();
+                a.n0 = a.n1 = V.node;
+                a.flag = 3;
+                const int kb = pp_kif_prop_bits(r.lo, r.hi, r.step); // the tracer's cost: half a LUT per bit for relu, and for a negation
+                a.q0[0] = (float)((V.f < 0 ? kb / 2.0 : 0.0) + (relu ? kb / 2.0 : 0.0));
+                if (split) {
+                    split->xv.insert(split->xv.end(), {V.lo, V.hi, V.step, V.f});
+                    split->yv.insert(split->yv.end(), {0.0, 0.0, 0.0, 0.0});
+                    split->x.push_back(V.node);
+                    split->y.push_back(-1);
+                    split->opc.push_back((V.f < 0 ? -1 : 1) * (relu ? 2 : 3));
+                    split->data.push_back(0);
+                }
+                node_view.push_back(View{a.node, r.lo, r.hi, r.step, std::fabs(V.f)});
+                lvl.push_back(1 + lvl[V.node]);
+                adds.push_back(a);
+                buf[i] = node_view.back();
+                continue;
+            }
             View A = buf[o[0]], B = scaled(buf[o[1]], std::ldexp(1.0, (int)o[3]));
             if (o[2] == 1)
-                B = scaled(B, -1.0);
+                B = negated(B);
             PpAdd a{};
             a.node = P.n_in + 1 + (int)adds.size();
             a.n0 = A.node;
             a.n1 = B.node;
             a.flag = (A.lo == A.hi || B.lo == B.hi) ? 2 : 0;
-            const double lo = A.lo + B.lo, hi = A.hi + B.hi, step = std::min(A.step, B.step);
-            double f = A.f;
             View X = A, Y = B; // FixedVariable.__add__: the operand with a positive factor first; both negative: negate both
+            bool neg = false;
             if (A.f < 0) {
                 if (B.f > 0)
-                    X = B, Y = A, f = B.f;
+                    X = B, Y = A;
                 else
-                    X = scaled(A, -1.0), Y = scaled(B, -1.0);
+                    X = negated(A), Y = negated(B), neg = true;
             }
+            // the new node is X + Y (factor X.f), seen negated when both operands were; in this order, as the tracer's
+            // Decimal arithmetic gives the signs of zero bounds (which reach the split's op intervals)
+            const double clo = X.lo + Y.lo, chi = X.hi + Y.hi, step = std::min(A.step, B.step);
+            const double lo = neg ? 0.0 - chi : clo, hi = neg ? 0.0 - clo : chi, f = neg ? -X.f : X.f;
             a.q0[0] = (float)X.lo, a.q0[1] = (float)X.hi, a.q0[2] = (float)X.step;
             a.q1[0] = (float)Y.lo, a.q1[1] = (float)Y.hi, a.q1[2] = (float)Y.step;
             if (split) {
+                split->xv.insert(split->xv.end(), {X.lo, X.hi, X.step, X.f});
+                split->yv.insert(split->yv.end(), {Y.lo, Y.hi, Y.step, Y.f});
                 split->x.push_back(X.node);
                 split->y.push_back(Y.node);
                 split->opc.push_back(Y.f < 0);
@@ -378,6 +512,7 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
             split->own_q[3 * v] = w.lo, split->own_q[3 * v + 1] = w.hi, split->own_q[3 * v + 2] = w.step;
         }
         for (const View &v : cur) {
+            split->out_v.insert(split->out_v.end(), {v.lo, v.hi, v.step, v.f});
             split->out_shift.push_back((int64_t)std::log2(std::fabs(v.f)));
             split->out_neg.push_back(v.f < 0);
         }

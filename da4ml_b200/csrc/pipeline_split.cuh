@@ -31,9 +31,10 @@ enum PsStatus : int { PS_SPLIT = 0, PS_NOT_OK = 1 /* the task is not ok: no spli
 struct PsItem {
     double lo, hi, step;  // the op's interval (the node's own)
     int node, gpos;       // node id (PpDesign) and position in gather_variables' list
-    int inp;              // >= 0: network input k; -1: adder; -2: constant (an all-zero output column)
-    int x, y, opc, data;  // adder: items of the operands in _from order, opcode, shift; input: opcode -1, or 5 and the
-                          // value in steps for an input with a point interval (a constant to the tracer)
+    int inp;              // >= 0: network input k; -1: adder; -2: constant (an all-zero output column); -3: activation
+    int x, y, opc, data;  // adder: items of the operands in _from order, opcode, shift; activation: the operand's item, y
+                          // -1, opcode +-2 / +-3, data 0; input: opcode -1, or 5 and the value in steps for an input with
+                          // a point interval (a constant to the tracer)
     int live;             // reachable from the outputs
 };
 
@@ -202,10 +203,10 @@ __global__ void __launch_bounds__(256) pipeline_split_kernel(const PsDesign *des
     // last consumer stage of every item: the stage of each adder reading it, and the output stage
     for (int i = tid; i < M; i += nt) {
         const PsItem &it = D.items[i];
-        if (it.inp == -1) {
+        if (it.inp == -1 || it.inp == -3)
             atomicMax(&t.last[it.x], t.stg[i]);
+        if (it.inp == -1)
             atomicMax(&t.last[it.y], t.stg[i]);
-        }
     }
     for (int o = tid; o < d.n_out; o += nt)
         atomicMax(&t.last[D.out_item[o]], s_out);
@@ -262,12 +263,12 @@ __global__ void __launch_bounds__(256) pipeline_split_write_kernel(const PsDesig
     // across every boundary below s: record it at the last one, a suffix min then gives each copy its first event
     for (int i = tid; i < M; i += nt) {
         const PsItem &it = D.items[i];
-        if (it.inp != -1)
+        if (it.inp != -1 && it.inp != -3)
             continue;
         const int s = stg[i];
         if (s > stg[it.x])
             atomicMin(&t.ev[coff[it.x] + s - 1 - stg[it.x]], 3 * rank[i]);
-        if (s > stg[it.y])
+        if (it.inp == -1 && s > stg[it.y])
             atomicMin(&t.ev[coff[it.y] + s - 1 - stg[it.y]], 3 * rank[i] + 1);
     }
     for (int o = tid; o < n_out; o += nt) {
@@ -328,7 +329,7 @@ __global__ void __launch_bounds__(256) pipeline_split_write_kernel(const PsDesig
             else if (it.inp == -2)
                 oi[0] = -1, oi[1] = -1, oi[2] = 5, oi[3] = 0;
             else {
-                oi[0] = where(it.x, s), oi[1] = where(it.y, s), oi[2] = it.opc, oi[3] = it.data;
+                oi[0] = where(it.x, s), oi[1] = it.inp == -1 ? where(it.y, s) : -1, oi[2] = it.opc, oi[3] = it.data;
                 cost = (double)t.cost[it.node];
             }
             of[0] = it.lo, of[1] = it.hi, of[2] = it.step, of[3] = t.pp.lat[it.node], of[4] = cost;
@@ -362,10 +363,17 @@ inline PsPrep ps_prepare(const PpPrepared &P, const PpSplitInfo &S) {
     PsPrep Q;
     const int CONST = P.n_in;
     std::vector<int> item_of(P.n_nodes, -1);
+    // an op's interval is FixedVariable.unscaled of the view gather_variables met the node through first (its bounds'
+    // signs of zero depend on that view's factor); own[node] is set when the walk enters the node
+    std::vector<double> own(S.own_q);
+    auto enter = [&](int node, const double *v) { // v: (lo, hi, step, factor); `self * (1 / factor)` in Decimal
+        const double o = 1.0 / v[3], a = v[0] * o, b = v[1] * o;
+        own[3 * (size_t)node] = std::min(a, b), own[3 * (size_t)node + 1] = std::max(a, b), own[3 * (size_t)node + 2] = std::fabs(v[2] * o);
+    };
     auto add_item = [&](int node, int gpos) {
         PsItem it{};
         it.node = node, it.gpos = gpos;
-        it.lo = S.own_q[3 * (size_t)node], it.hi = S.own_q[3 * (size_t)node + 1], it.step = S.own_q[3 * (size_t)node + 2];
+        it.lo = own[3 * (size_t)node], it.hi = own[3 * (size_t)node + 1], it.step = own[3 * (size_t)node + 2];
         it.inp = node < P.n_in ? node : node == CONST ? -2 : -1;
         it.x = it.y = -1;
         it.opc = -1;
@@ -386,8 +394,10 @@ inline PsPrep ps_prepare(const PpPrepared &P, const PpSplitInfo &S) {
         }
         if (it.inp == -1) {
             const int a = node - P.n_in - 1;
-            it.x = item_of[S.x[a]], it.y = item_of[S.y[a]];
+            it.x = item_of[S.x[a]], it.y = S.y[a] < 0 ? -1 : item_of[S.y[a]];
             it.opc = S.opc[a], it.data = S.data[a];
+            if (S.y[a] < 0) // relu / quantize
+                it.inp = -3;
         }
         Q.items.push_back(it);
         return (int)Q.items.size() - 1;
@@ -398,18 +408,25 @@ inline PsPrep ps_prepare(const PpPrepared &P, const PpSplitInfo &S) {
     std::vector<char> seen(P.n_nodes, 0);
     for (int k = 0; k < P.n_in; ++k)
         seen[k] = 1;
-    std::vector<std::pair<int, bool>> stack;
+    struct Entry {
+        int node;
+        bool done;
+        const double *view;
+    };
+    std::vector<Entry> stack;
+    std::vector<char> entered(P.n_nodes, 0);
     for (int o = 0; o < P.n_out; ++o) {
         const int root = P.out_node[o];
         if (root == CONST) { // a fresh constant for every all-zero column
             Q.out_item.push_back(add_item(CONST, pos++));
             continue;
         }
-        stack.assign(1, {root, false});
+        stack.assign(1, {root, false, S.out_v.data() + 4 * (size_t)o});
         while (!stack.empty()) {
-            const auto [v, done] = stack.back();
+            const Entry e = stack.back();
+            const int v = e.node;
             stack.pop_back();
-            if (done) {
+            if (e.done) {
                 if (!seen[v]) {
                     seen[v] = 1;
                     item_of[v] = add_item(v, pos++);
@@ -418,11 +435,16 @@ inline PsPrep ps_prepare(const PpPrepared &P, const PpSplitInfo &S) {
             }
             if (seen[v])
                 continue;
-            stack.push_back({v, true});
+            if (!entered[v]) {
+                entered[v] = 1;
+                enter(v, e.view);
+            }
+            stack.push_back({v, true, nullptr});
             if (v > CONST) {
                 const int a = v - P.n_in - 1;
-                stack.push_back({S.y[a], false});
-                stack.push_back({S.x[a], false});
+                if (S.y[a] >= 0)
+                    stack.push_back({S.y[a], false, S.yv.data() + 4 * (size_t)a});
+                stack.push_back({S.x[a], false, S.xv.data() + 4 * (size_t)a});
             }
         }
         Q.out_item.push_back(item_of[root]);

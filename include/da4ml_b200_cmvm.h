@@ -228,8 +228,10 @@ int da4ml_pipeline_profile(const da4ml_pipeline_t *p, double out[8]);
  * split), latency_max (the traced output latencies' maximum), cutoff_out (the cutoff retiming settled on; the cutoff
  * itself without retiming); out_latency (NULL to skip) [n_designs][n_cutoffs][n_out of the design] the traced output
  * latencies (0.0 for a dead column).  Not ok: stages = reg_bits = -1, latencies NaN.  profile (NULL to skip) =
- * {device_ms, launches}.  Arguments are checked on the host before any device call: shapes, opcodes other than -1/0/1,
- * operands and cutoffs <= 0 give DA4ML_E_INVALID. */
+ * {device_ms, launches}.  A design may also hold the relu / quantize ops of a chain design (opcodes +-2 / +-3: id0 an
+ * earlier op, id1 -1, data 0, the op's interval on a power-of-two grid giving its (k, i, f); TRN / WRAP), replayed as
+ * CombLogic.__call__ replays them.  Arguments are checked on the host before any device call: shapes, other opcodes,
+ * operands, bad activation intervals, an activation of a non-zero constant and cutoffs <= 0 give DA4ML_E_INVALID. */
 int da4ml_pipeline_price(
     int64_t n_designs, const int64_t *n_stages, const int64_t *stage_meta, const int64_t *inp_shifts,
     const int64_t *out_idxs, const int64_t *out_shifts, const int64_t *out_negs, const int64_t *ops_i,
@@ -243,7 +245,8 @@ int da4ml_pipeline_price(
  * op tables copied back}, and *out a handle to free with da4ml_split_free.  The split of task (d, j) is what the
  * reference's to_pipeline(comb, c, retiming) returns: without retiming, the split of the trace under d's input latencies;
  * with it, retime_pipeline's (the first split when no bisection round succeeded, else the last successful round's, at
- * cutoff_out with every input at latency 0).  Arguments are checked on the host before any device call. */
+ * cutoff_out with every input at latency 0).  Relu / quantize ops come back as the tracer writes them: (id0, -1, +-2 / +-3,
+ * 0), negative for a negated operand.  Arguments are checked on the host before any device call. */
 typedef struct da4ml_split da4ml_split_t; /* opaque split result */
 int da4ml_pipeline_split(
     int64_t n_designs, const int64_t *n_stages, const int64_t *stage_meta, const int64_t *inp_shifts,
