@@ -12,6 +12,7 @@ from __future__ import annotations
 
 import copy
 import ctypes as C
+import time
 from collections import namedtuple
 from pathlib import Path
 
@@ -715,12 +716,19 @@ class ChainFront(NetworkFront):
     latencies.  ``best(latency_budget)`` is ``NetworkFront.best``.  ``profile`` holds the sweeps' launches, device time
     and jobs, in total and per layer (``layers[k]``: input-latency states, candidates, points kept, ...).
 
+    ``activations``: the relu / quantizers between the layers that the front was searched with (``chain_front(...,
+    activations=...)``, each as ``(kind, [n_out, 3] kif)``), or ``None``.
+
     Only host arrays are held (each point's designs are ``RawPipeline`` copies), so a front pickles as it is."""
 
-    def __init__(self, cost, latency, choice, raws, calls, profile, latency_cutoff=0.0):
+    activations = None  # (a front built without activations holds no attribute of its own: it pickles as before)
+
+    def __init__(self, cost, latency, choice, raws, calls, profile, latency_cutoff=0.0, activations=None):
         super().__init__(cost, latency, choice)
         self._raws, self._calls, self.profile = raws, calls, profile
         self.latency_cutoff = float(latency_cutoff)
+        if activations is not None:
+            self.activations = activations
         c = self.latency_cutoff
         # (to_pipeline's stage of the last output, + 1: the clock count of a chain whose network inputs arrive before c)
         self.stages = (np.floor(np.asarray(latency, np.float64) / (c + 1e-9)).astype(np.int64) + 1) if c > 0 else np.ones(len(cost), np.int64)
@@ -742,20 +750,36 @@ class ChainFront(NetworkFront):
         """Point ``p``'s designs as one ``Pipeline`` per layer."""
         return [r.to_pipeline(types_module) for r in self._raws[p]]
 
-    def design(self, p: int, activations) -> RawPipeline:
+    def design(self, p: int, activations=None) -> RawPipeline:
         """Point ``p``'s designs as one chain design with ``activations`` between the layers: ``chain_design(self.pipelines(p),
-        activations)``, for ``price_pipelined`` (register bits, ``keep_split``)."""
+        activations)``, for ``price_pipelined`` (register bits, ``keep_split``).  A front searched with activations uses its
+        own when none are given, and refuses others (``ValueError``): its later layers were solved for its own.  A front
+        searched without them needs them."""
+        if activations is None:
+            if self.activations is None:
+                raise TypeError('this front was searched without activations: design(p, activations) needs them')
+            activations = self.activations
+        elif self.activations is not None:
+            acts = list(activations)
+            same = len(acts) == len(self.activations)
+            for k, (act, (kind, kif)) in enumerate(zip(acts, self.activations) if same else ()):
+                a_kind, a_kif = _act_arg(k, act, len(kif))
+                same &= a_kind == kind and np.array_equal(a_kif, kif)
+            if not same:
+                raise ValueError('these activations differ from the ones the front was searched with: its later layers were solved for those')
         return chain_design(self._raws[p], activations)
 
     def reference_calls(self, p: int) -> list[dict]:
         """Per layer, the keywords of the ``solve(kernels[k], **kw)`` call that returns layer ``k``'s design in point
         ``p``: the candidate's options, the layer's ``qintervals`` and its input ``latencies`` as Python floats (for
-        ``k > 0``, the output latencies of the point's design of layer ``k - 1``).  A candidate of a seeded option set
-        carries its ``seed``, as ``SweepResult.reference_call`` does."""
+        ``k > 0``, the output latencies of the point's design of layer ``k - 1``).  With activations, ``qintervals`` of
+        ``k > 0`` are the intervals of layer ``k - 1``'s traced outputs after the activation, as the float32 values the
+        layer was solved under.  A candidate of a seeded option set carries its ``seed``, as ``SweepResult.reference_call``
+        does."""
         return copy.deepcopy(self._calls[p])
 
 
-def _chain_layer(points, state_of, sweeps, state_lats, traced=None):
+def _chain_layer(points, state_of, sweeps, state_lats, traced=None, state_qs=None, acted=None):
     """Extend the points of the layers so far by the next layer and prune.  ``points`` is ``None`` at layer 0, else
     ``(cost, lat, choice, outs, raws, calls)``; ``state_of[p]`` is the index of point ``p``'s input-latency state in
     ``sweeps`` and ``state_lats`` (lists of Python floats); at layer 0 there is one state and ``state_of == [0]``.
@@ -763,7 +787,15 @@ def _chain_layer(points, state_of, sweeps, state_lats, traced=None):
     order; cost is the float32 sum in layer order, latency the new design's ``latency_max``; then the ``sweep_front``
     rule.  ``outs[p]`` are the output latencies of point ``p``'s last design.  ``traced[s, i]`` (pipelined chains):
     ``(latency_max, output latencies)`` of front candidate ``i`` of state ``s`` as traced under the cutoff, which replace the
-    solver's; a front candidate without an entry is dropped."""
+    solver's; a front candidate without an entry is dropped.
+
+    Chains with activations: ``state_qs[s]`` are state ``s``'s qintervals for the reference calls, and ``acted`` is
+    ``(group_of, table)`` at every layer but the last: ``group_of[p]`` is parent ``p``'s replay group (the parents of one state with the same float64
+    input intervals); ``table[g, i]`` is ``None`` when candidate ``i`` under group ``g`` makes a non-zero constant (the
+    pair is dropped), else ``(act_cost, zero, intervals)``: the float32 cost of each output's activation op (0 without
+    one), which outputs become the constant 0, and the outputs' intervals after the activation.  A point's cost then
+    continues with ``act_cost`` added in output order, and its ``outs`` entry is ``(latencies, intervals)``, the latency
+    of a constant 0 being 0."""
     fronts = [np.asarray(sw.front, np.int64) for sw in sweeps]
     if traced is not None:
         fronts = [np.asarray([i for i in f.tolist() if (s, i) in traced], np.int64) for s, f in enumerate(fronts)]
@@ -777,8 +809,16 @@ def _chain_layer(points, state_of, sweeps, state_lats, traced=None):
     cand = np.concatenate([fronts[s] for s in state_of])
     cost = np.concatenate([f_cost[s] for s in state_of])
     lat = np.concatenate([f_lat[s] for s in state_of])
+    if acted is not None:
+        group_of, table = acted
+        ok = np.asarray([table[group_of[p], i] is not None for p, i in zip(par.tolist(), cand.tolist())], bool).reshape(-1)
+        par, sidx, cand, cost, lat = par[ok], sidx[ok], cand[ok], cost[ok], lat[ok]
     if points is not None:
         cost = points[0][par] + cost
+    if acted is not None and par.size:
+        act_cost = np.stack([table[group_of[p], i][0] for p, i in zip(par.tolist(), cand.tolist())])
+        for j in range(act_cost.shape[1]):  # (float32, in output order: the order of the activation stage's ops)
+            cost = cost + act_cost[:, j]
     keep = sweep_front(cost, lat)
     par, sidx, cand, cost, lat = par[keep], sidx[keep], cand[keep], cost[keep], lat[keep]
     choice = cand[:, None] if points is None else np.concatenate([points[2][par], cand[:, None]], axis=1)
@@ -787,15 +827,22 @@ def _chain_layer(points, state_of, sweeps, state_lats, traced=None):
     for p, s, i in zip(par.tolist(), sidx.tolist(), cand.tolist()):
         if (s, i) not in designs:
             r = sweeps[s].raw(i)
-            designs[s, i] = (r, {**sweeps[s].reference_call(i), 'latencies': state_lats[s]}, _out_latencies(r) if traced is None else traced[s, i][1])
+            call = {**sweeps[s].reference_call(i), 'latencies': state_lats[s]}
+            if state_qs is not None:
+                call['qintervals'] = state_qs[s]
+            designs[s, i] = (r, call, _out_latencies(r) if traced is None else traced[s, i][1])
         r, call, o = designs[s, i]
         raws.append([r] if points is None else [*points[4][p], r])
         calls.append([call] if points is None else [*points[5][p], call])
+        if acted is not None:
+            _, zero, vals = table[group_of[p], i]
+            o = (np.where(zero, 0.0, o).astype(o.dtype), vals)
         outs.append(o)
     return cost, lat, choice, outs, raws, calls
 
 
-def chain_front(kernels, option_sets, qintervals=None, latencies=None, adder_size=-1, carry_size=-1, solver=None, latency_cutoff=0.0, pricer=None) -> ChainFront:
+def chain_front(kernels, option_sets, qintervals=None, latencies=None, adder_size=-1, carry_size=-1, solver=None, latency_cutoff=0.0, pricer=None,
+                activations=None) -> ChainFront:
     """The cost / latency front of a chain of layers, each layer solved under the output latencies of the design chosen
     for the layer before it, as a traced model's matmuls are: every reported design is what
     ``solve(kernels[k], **front.reference_calls(p)[k])`` returns, and every reported cost and latency is the chain's own.
@@ -803,16 +850,27 @@ def chain_front(kernels, option_sets, qintervals=None, latencies=None, adder_siz
     ``kernels[k]`` is layer ``k``'s constant matrix (``kernels[k].shape[1] == kernels[k + 1].shape[0]``).
     ``option_sets`` and the cost model (``adder_size``, ``carry_size``) are those of ``solve_sweep`` and the same for
     every layer.  ``qintervals`` is ``None`` or one entry per layer: ``None`` (``solve``'s default) or that layer's input
-    intervals, e.g. those of the quantizer in front of it; intervals are not carried over from a layer's outputs.
-    ``latencies`` are layer 0's input latencies (default zeros).
+    intervals, e.g. those of the quantizer in front of it; without ``activations``, intervals are not carried over from a
+    layer's outputs.  ``latencies`` are layer 0's input latencies (default zeros).
+
+    ``activations[k]`` (``len(kernels) - 1`` of them, in ``chain_design``'s format: ``('relu' | 'quantize', kif[, 'TRN'[,
+    'WRAP']])``) is the op between layer ``k`` and layer ``k + 1``.  With them every layer after the first is solved under
+    the intervals a traced model hands it: those of the previous design's traced outputs after the activation (the
+    intervals ``chain_design`` gives the activation stage's outputs).  A dead column, or a value that loses all its bits, is
+    the tracer's constant 0: the interval (0, 0, 2**32) at latency 0.  Only ``qintervals[0]`` may then be given (``ValueError`` otherwise).
 
     Search: layer 0 is swept once, and its ``front`` candidates are the first points.  At each later layer a point's
     input-latency state is the output latencies of its last design (``Pipeline.out_latencies``; 0.0 for a constant-zero
-    output); points whose states are equal as float32 share one problem, and all the layer's states go into one
-    ``solver`` call (``solve_sweep_batch``: one GPU pass per layer).  Each point is extended by every ``front`` candidate
+    output), with activations together with its activated intervals; points whose states are equal as float32 (the values
+    the solver sees) share one problem, and all the layer's states go into one ``solver`` call (``solve_sweep_batch``:
+    one GPU pass per layer, each state with its own ``qintervals``).  Each point is extended by every ``front`` candidate
     of its state's sweep; its cost is the float32 sum of the designs' costs in layer order, and its latency the new
-    design's ``latency_max``, which already contains the upstream latency.  The points are pruned after each layer with
-    the ``sweep_front`` rule, and the result is sorted by ascending latency.
+    design's ``latency_max``, which already contains the upstream latency.  With activations the cost is the float32 sum,
+    in stage order, of the ``ops_f`` cost column of the point's chain design (``design(p)``): each layer design's cost
+    followed by the cost of each op of the activation after it, in output order (relu: ``sum(kif) / 2`` per changed
+    value, quantize: 0).  A (state, candidate) pair whose activation turns some output into a non-zero constant is
+    dropped (``profile['layers'][k]['dropped_constant']``; ``replay_ms`` is the host time of the interval replay).  The
+    points are pruned after each layer with the ``sweep_front`` rule, and the result is sorted by ascending latency.
 
     Latency model: with ``latency_cutoff = 0`` (the default) latency is the solver's op latency.  With ``latency_cutoff =
     c > 0`` it is the latency the tracer gives the design under ``HWConfig(adder_size, carry_size, c)``: after each
@@ -843,6 +901,15 @@ def chain_front(kernels, option_sets, qintervals=None, latencies=None, adder_siz
     sets = _sweep_sets(option_sets)
     if qintervals is not None and len(qintervals) != len(ks):
         raise ValueError(f'expected qintervals for {len(ks)} layers, got {len(qintervals)}')
+    acts = None
+    if activations is not None:
+        acts = list(activations)
+        if len(acts) != len(ks) - 1:
+            raise ValueError(f'{len(ks)} layers need {len(ks) - 1} activations, got {len(acts)}')
+        acts = [_act_arg(k, act, int(ks[k].shape[1])) for k, act in enumerate(acts)]
+        for k in range(1, len(ks) if qintervals is not None else 0):
+            if qintervals[k] is not None:
+                raise ValueError(f"layer {k}: with activations a layer's qintervals are its traced inputs' (only layer 0's may be given)")
     qs = [None if qintervals is None else _prefixed(f'layer {k}', _qint_arg, qintervals[k], W.shape[0]) for k, W in enumerate(ks)]
     qs = [None if q is None else [tuple(map(float, r)) for r in q] for q in qs]
     l0 = _prefixed('layer 0', _lat_arg, latencies, ks[0].shape[0])
@@ -851,36 +918,87 @@ def chain_front(kernels, option_sets, qintervals=None, latencies=None, adder_siz
         raise ValueError(f'latency_cutoff must be a non-negative number, got {latency_cutoff!r}')
     dt = np.float64 if c > 0 else np.float32  # (traced latencies are the tracer's doubles)
     states = [np.zeros(ks[0].shape[0], dt) if l0 is None else l0.astype(dt)]
+    state_qs = [qs[0]]  # (with activations: each state's qintervals, float32 values as Python floats)
     solver = solve_sweep_batch if solver is None else solver
     pricer = price_pipelined if pricer is None else pricer
     prof = dict(launches=0, device_ms=0.0, jobs_run=0, jobs_total=0, layers=[])
     points, state_of = None, np.zeros(1, np.int64)
     for k, W in enumerate(ks):
-        if k > 0:  # one state per distinct output-latency vector, in order of first use
+        if k > 0 and acts is None:  # one state per distinct output-latency vector, in order of first use
             index = {}
             state_of = np.asarray([index.setdefault(np.asarray(o, dt).tobytes(), len(index)) for o in points[3]], np.int64)
             states = [np.frombuffer(b, dt) for b in index]
+        elif k > 0:  # one state per distinct (output latencies, float32 activated intervals), in order of first use
+            index, first = {}, []
+            for p, (o, v) in enumerate(points[3]):
+                key = np.asarray(o, dt).tobytes() + np.asarray(v, np.float32).tobytes()
+                if key not in index:
+                    index[key] = len(first)
+                    first.append(p)
+            state_of = np.asarray([index[np.asarray(o, dt).tobytes() + np.asarray(v, np.float32).tobytes()] for o, v in points[3]], np.int64)
+            states = [np.asarray(points[3][p][0], dt) for p in first]
+            state_qs = [[tuple(map(float, r)) for r in np.asarray(points[3][p][1], np.float32)] for p in first]
         n, lats = len(states), [[float(v) for v in s] for s in states]
-        sweeps = _prefixed(f'layer {k}', solver, [W] * n, sets, qintervals=[qs[k]] * n, latencies=lats, adder_size=int(adder_size), carry_size=int(carry_size))
+        sweeps = _prefixed(f'layer {k}', solver, [W] * n, sets, qintervals=[qs[k]] * n if acts is None else state_qs, latencies=lats, adder_size=int(adder_size),
+                           carry_size=int(carry_size))  # fmt: skip
         traced, priced = None, {}
         if c > 0:  # every front candidate of every state, traced under its state's latencies: one pricing call
             keys = [(s, int(i)) for s, sw in enumerate(sweeps) for i in np.asarray(sw.front, np.int64).tolist()]
             pr = _prefixed(f'layer {k}', pricer, [sweeps[s].raw(i) for s, i in keys], c, latencies=[lats[s] for s, _ in keys], retiming=False)
             traced = {key: (float(pr.latency_max[j, 0]), np.asarray(pr.out_latency(j, 0), np.float64)) for j, key in enumerate(keys) if int(pr.status[j, 0]) == 0}
             priced = dict(dropped=len(keys) - len(traced), price_launches=int(pr.profile.get('launches', 0)), price_device_ms=float(pr.profile.get('device_ms', 0.0)))
-        points = _chain_layer(points, state_of, sweeps, lats, traced)
+        acted, replayed = None, {}
+        if acts is not None and k < len(ks) - 1:
+            t0 = time.perf_counter()
+            acted = _chain_replay(points, state_of, sweeps, traced, k, *acts[k])
+            replayed = dict(replay_ms=(time.perf_counter() - t0) * 1e3, dropped_constant=sum(v is None for v in acted[1].values()))
+        elif acts is not None:
+            replayed = dict(replay_ms=0.0, dropped_constant=0)
+        points = _chain_layer(points, state_of, sweeps, lats, traced, None if acts is None else state_qs, acted)
         if len(points[0]) == 0:
+            if replayed.get('dropped_constant'):
+                raise ValueError(f'layer {k}: every front candidate is slower than the latency cutoff {c} or makes an output of activation {k} a non-zero constant')
             raise ValueError(f'layer {k}: every front candidate has an adder slower than the latency cutoff {c}')
         p0 = sweeps[0].profile  # (the whole call's)
         layer = dict(states=n, candidates=sum(len(sw.candidates['cost']) for sw in sweeps), points=len(points[0]),
-                     **{key: p0[key] for key in ('launches', 'device_ms', 'jobs_run', 'jobs_total')}, **priced)
+                     **{key: p0[key] for key in ('launches', 'device_ms', 'jobs_run', 'jobs_total')}, **priced, **replayed)
         prof['layers'].append(layer)
         for key in ('launches', 'device_ms', 'jobs_run', 'jobs_total'):
             prof[key] += layer[key]
         del sweeps  # (the designs are copied out: free the handles before the next layer's call)
     cost, lat, choice, _, raws, calls = points
     order = np.argsort(lat, kind='stable')
-    return ChainFront(cost[order], lat[order], choice[order], [raws[p] for p in order], [calls[p] for p in order], prof, c)
+    return ChainFront(cost[order], lat[order], choice[order], [raws[p] for p in order], [calls[p] for p in order], prof, c, acts)
+
+
+_ZERO_QINT = (0.0, 0.0, 2.0**32)  # the tracer's constant 0: FixedVariable gives a constant the step 2**-_const_f(0) = 2**32
+
+
+def _chain_replay(points, state_of, sweeps, traced, k, kind, kif):
+    """``_chain_layer``'s ``acted`` for layer ``k`` of a chain with activations: every front candidate (that pricing
+    kept) of every state, replayed through activation ``k`` from each distinct float64 input intervals of the state's
+    parents (at layer 0, the design's own input intervals, as in ``chain_design``)."""
+    group_of, groups = [], {}  # parent -> replay group; (state, float64 intervals) -> group
+    for p, s in enumerate(state_of.tolist()):
+        vin = None if points is None else np.asarray(points[3][p][1], np.float64)
+        group_of.append(groups.setdefault((s, None if vin is None else vin.tobytes()), len(groups)))
+    table = {}
+    for (s, vb), g in groups.items():
+        for i in np.asarray(sweeps[s].front, np.int64).tolist():
+            if traced is not None and (s, i) not in traced:
+                continue
+            stages = sweeps[s].raw(i).stages
+            vals = _input_intervals(stages) if vb is None else [tuple(r) for r in np.frombuffer(vb, np.float64).reshape(-1, 3).tolist()]
+            try:
+                traced_vals, changed = _activated_intervals(stages, vals, k, kind, kif)
+            except _ConstantValue:
+                table[g, i] = None
+                continue
+            act_cost = np.asarray([0.0 if a is None else a[3] for a in changed], np.float32)
+            zero = np.asarray([a is not None and a[0] == a[1] for a in changed], bool)
+            vals = [t if a is None else _ZERO_QINT if a[0] == a[1] else a[:3] for t, a in zip(traced_vals, changed)]
+            table[g, i] = (act_cost, zero, np.asarray(vals, np.float64).reshape(-1, 3))
+    return group_of, table
 
 
 def _kif_prop(lo: float, hi: float, step: float) -> tuple[int, int, int]:
@@ -944,6 +1062,49 @@ def _traced_intervals(stages, vals):
             lo, hi, s = (v * 2.0**sh for v in buf[i])
             vals.append((-hi, -lo, s) if ng else (lo, hi, s))
     return vals
+
+
+class _ConstantValue(ValueError):
+    """A value of a chain that is or becomes a constant other than 0: ``chain_design`` refuses it, ``chain_front`` drops
+    the candidate."""
+
+
+def _input_intervals(stages) -> list:
+    """The intervals (lo, hi, step) of a design's inputs (``CombLogic.inp_qint``: an input without an input op is (0, 0, 1))."""
+    s0 = stages[0]
+    vals = [(0.0, 0.0, 1.0)] * int(s0['shape'][0])
+    for (id0, _, opc, _), q in zip(np.asarray(s0['ops_i'], np.int64).reshape(-1, 4).tolist(), np.asarray(s0['ops_f'], np.float64).reshape(-1, 5).tolist()):
+        if opc == -1:
+            vals[id0] = tuple(q[:3])
+    return vals
+
+
+def _activated_intervals(stages, vals, k: int, kind: str, kif):
+    """One step of the tracer's interval replay of a chain: layer ``k``'s design (``stages``) on inputs of intervals
+    ``vals`` (``_traced_intervals``), then activation ``k`` (``kind``, ``[n_out, 3]`` kif) on every output.  Returns
+    ``(traced, acts)``: ``traced[j]`` is output ``j``'s (lo, hi, step); ``acts[j]`` is ``None`` when the activation leaves it
+    unchanged, else the (lo, hi, step, cost) of the op the tracer records for it (cost ``sum(kif) / 2`` for relu, 0 for
+    quantize), or (0.0, 0.0, 1.0, 0.0) for the constant 0 (a dead column, or a format with no bits left).
+    ``_ConstantValue`` when a value is or becomes any other constant.  The one Python copy of these rules (the C++ copy
+    is ``pp_prepare``'s)."""
+    traced = _traced_intervals(stages, vals)
+    acts = []
+    for j, (lo, hi, st) in enumerate(traced):
+        if lo == hi:
+            if lo != 0.0 or hi != 0.0:
+                raise _ConstantValue(f'activation {k}: output {j} of layer {k} is the constant {lo} (only the constant 0 is covered)')
+            acts.append((0.0, 0.0, 1.0, 0.0))
+            continue
+        r = _activate(kind, lo, hi, st, *(int(v) for v in kif[j]))
+        if r is None:
+            acts.append(None)
+        elif r[0] == r[1]:
+            if r[0] != 0.0:
+                raise _ConstantValue(f'activation {k}: output {j} becomes the constant {r[0]} (only the constant 0 is covered)')
+            acts.append((0.0, 0.0, 1.0, 0.0))
+        else:
+            acts.append((*r, sum(_kif_prop(*r)) / 2 if kind == 'relu' else 0.0))
+    return traced, acts
 
 
 def _act_arg(k: int, act, n: int):
@@ -1011,42 +1172,27 @@ def chain_design(designs, activations) -> RawPipeline:
         if stages[k - 1][-1]['shape'][1] != stages[k][0]['shape'][0]:
             raise ValueError(f"layer {k - 1} has {stages[k - 1][-1]['shape'][1]} outputs but layer {k} has {stages[k][0]['shape'][0]} inputs")
     kinds = [_act_arg(k, act, int(stages[k][-1]['shape'][1])) for k, act in enumerate(acts)]
-    s0 = stages[0][0]
-    vals = [(0.0, 0.0, 1.0)] * int(s0['shape'][0])  # (CombLogic.inp_qint)
-    for (id0, _, opc, _), q in zip(np.asarray(s0['ops_i'], np.int64).reshape(-1, 4).tolist(), np.asarray(s0['ops_f'], np.float64).reshape(-1, 5).tolist()):
-        if opc == -1:
-            vals[id0] = tuple(q[:3])
+    vals = _input_intervals(stages[0])
     out = [dict(st) for st in stages[0]]
     for k, (kind, kif) in enumerate(kinds):
         last = stages[k][-1]
         n = int(last['shape'][1])
-        vals = _traced_intervals(stages[k], vals)
+        traced, changed = _activated_intervals(stages[k], vals, k, kind, kif)
         idx = np.asarray(last['out_idxs'], np.int64)
         of = np.asarray(last['ops_f'], np.float64).reshape(-1, 5)
         ops_i, ops_f, out_idxs = [], [], np.zeros(n, np.int64)
         for j in range(n):  # the input ops first, in value order: the traced interval and the solver's latency
             ops_i.append([j, -1, -1, 0])
-            ops_f.append([*vals[j], float(of[idx[j], 3]) if idx[j] >= 0 else 0.0, 0.0])
-        for j in range(n):
-            lo, hi, st, lat = ops_f[j][0], ops_f[j][1], ops_f[j][2], ops_f[j][3]
-            if idx[j] < 0 or lo == hi:
-                if lo != 0.0 or hi != 0.0:
-                    raise ValueError(f'activation {k}: output {j} of layer {k} is the constant {lo} (only the constant 0 is covered)')
-                out_idxs[j] = -1
-                continue
-            r = _activate(kind, lo, hi, st, *(int(v) for v in kif[j]))
-            if r is None:
+            ops_f.append([*traced[j], float(of[idx[j], 3]) if idx[j] >= 0 else 0.0, 0.0])
+        for j, a in enumerate(changed):
+            if a is None:
                 out_idxs[j] = j
-                continue
-            if r[0] == r[1]:
-                if r[0] != 0.0:
-                    raise ValueError(f'activation {k}: output {j} becomes the constant {r[0]} (only the constant 0 is covered)')
+            elif a[0] == a[1]:  # (the constant 0)
                 out_idxs[j] = -1
-                continue
-            cost = sum(_kif_prop(*r)) / 2 if kind == 'relu' else 0.0
-            out_idxs[j] = len(ops_i)
-            ops_i.append([j, -1, 2 if kind == 'relu' else 3, 0])
-            ops_f.append([*r, lat, cost])
+            else:
+                out_idxs[j] = len(ops_i)
+                ops_i.append([j, -1, 2 if kind == 'relu' else 3, 0])
+                ops_f.append([*a[:3], ops_f[j][3], a[3]])
         vals = [tuple(ops_f[i][:3]) if i >= 0 else (0.0, 0.0, 1.0) for i in out_idxs.tolist()]
         out.append(dict(shape=(n, n), inp_shifts=np.zeros(n, np.int64), out_idxs=out_idxs, out_shifts=np.zeros(n, np.int64), out_negs=np.zeros(n, np.int64),
                         ops_i=np.asarray(ops_i, np.int64).reshape(-1, 4), ops_f=np.asarray(ops_f, np.float32).reshape(-1, 5), adder_size=a_sz, carry_size=c_sz))

@@ -4,7 +4,8 @@
 GPU-side additions for many independent matrices, ``solve_sweep`` for one matrix under many option sets,
 ``solve_sweep_batch`` for many matrices under many option sets, ``network_front`` for the cheapest per-layer choice of a
 chain of layers under a latency budget, and ``chain_front`` for the same with each layer solved under the output latencies
-of the design before it (the designs and latencies a traced model gets).  ``solve``'s ``seed`` keyword picks the
+of the design before it (the designs and latencies a traced model gets; with ``activations=`` also under the intervals
+the relu / quantizers between the layers hand each layer).  ``solve``'s ``seed`` keyword picks the
 tie-break order of the greedy pair selection (0 = the reference's), and ``solve_best_of`` keeps the cheapest of many seeds.
 ``price_pipelined`` prices designs as they will be pipelined under a latency cutoff: clock stages, register bits and the
 tracer's latencies; ``chain_design`` joins a chain's designs, with the relu / quantizers between its layers, into one
