@@ -10,6 +10,7 @@ The shared library is the product's only compute path; importing this module wit
 
 from __future__ import annotations
 
+import contextlib
 import copy
 import ctypes as C
 import time
@@ -41,6 +42,7 @@ _L.da4ml_cmvm_plan.argtypes = [_i64p, C.c_int64, C.c_int, C.c_int, _i64p]
 _L.da4ml_cmvm_set_group_size.argtypes = [C.c_int]
 _L.da4ml_cmvm_set_accounting.argtypes = [C.c_int]
 _L.da4ml_cmvm_set_job_sharing.argtypes = [C.c_int]
+_L.da4ml_cmvm_set_capacity_override.argtypes = [_i64p]
 _L.da4ml_cmvm_solve.argtypes = [_f32p, C.c_int64, C.c_int64, C.c_char_p, C.c_char_p, C.c_int, C.c_int, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.POINTER(_vp)]
 _L.da4ml_cmvm_solve_batch.argtypes = [C.c_int64, C.POINTER(_f32p), _i64p, _i64p, C.c_char_p, C.c_char_p, C.c_int, C.c_int, C.POINTER(_f32p), C.POINTER(_f32p), C.c_int, C.c_int, C.c_int, C.POINTER(_vp)]
 _L.da4ml_cmvm_solve_batch_device.argtypes = [C.c_int64, C.POINTER(_vp), _i64p, _i64p, C.c_char_p, C.c_char_p, C.c_int, C.c_int, C.POINTER(_f32p), C.POINTER(_f32p), C.c_int, C.c_int, C.c_int, C.POINTER(_vp)]
@@ -107,7 +109,7 @@ EXPORTED_SYMBOLS = [
     'da4ml_dais_program_free', 'da4ml_dais_program_profile', 'da4ml_dais_program_dump', 'da4ml_cmvm_solve_sweep', 'da4ml_cmvm_solve_sweep_batch', 'da4ml_sweep_counts',
     'da4ml_sweep_profile', 'da4ml_sweep_summary', 'da4ml_sweep_pipeline', 'da4ml_sweep_free', 'da4ml_sweep_front',
     'da4ml_cmvm_solve_seeded', 'da4ml_cmvm_solve_single_seeded', 'da4ml_cmvm_solve_sweep_batch_seeded', 'da4ml_pipeline_price',
-    'da4ml_pipeline_split', 'da4ml_split_info', 'da4ml_split_copy', 'da4ml_split_free',
+    'da4ml_pipeline_split', 'da4ml_split_info', 'da4ml_split_copy', 'da4ml_split_free', 'da4ml_cmvm_set_capacity_override',
 ]  # fmt: skip
 
 COUNTER_NAMES = ['status', 'n_ops', 'T', 'sum_F', 'sum_R', 'F0', 'R0', 'D_final', 'F_max', 'compactions', 'D0', 'n_bits', 'group_ctas',
@@ -173,6 +175,32 @@ def set_job_sharing(on: bool):
 def set_accounting(on: bool):
     """Exact work counters (sum over iterations of the live histogram size); slower, identical results."""
     _L.da4ml_cmvm_set_accounting(int(bool(on)))
+
+
+CAPACITY_KNOBS = ['segment_entries', 'list_rows', 'spill_rows', 'hash_log', 'wide_rows', 'expr_cap', 'cell_pool', 'poison']
+
+
+@contextlib.contextmanager
+def capacity_override(**caps):
+    """Test-only: squeeze the solve kernel's capacities inside the ``with`` block, so that small problems reach its spill,
+    multi-pass, compaction, overflow and retry paths (``da4ml_cmvm_set_capacity_override``).  Knobs (``CAPACITY_KNOBS``,
+    omitted = the planner's): ``segment_entries`` histogram entries per CTA, ``list_rows`` shared-memory rows per owner
+    list (0: every row spills), ``spill_rows``, ``hash_log`` (8..13), ``wide_rows`` (bool), ``expr_cap`` expression ids
+    beyond the inputs, ``cell_pool`` cells per CTA, ``poison`` (bool: 0xA5 in every buffer the driver does not clear).
+    A knob only lowers the planner's value and grows with its retries; results must not change.  Every knob is reset on
+    exit."""
+    bad = set(caps) - set(CAPACITY_KNOBS)
+    if bad:
+        raise TypeError(f'unknown capacity knobs {sorted(bad)}; known: {CAPACITY_KNOBS}')
+    v = np.full(len(CAPACITY_KNOBS), -1, np.int64)
+    for k, x in caps.items():
+        if x is not None:
+            v[CAPACITY_KNOBS.index(k)] = (1 if x else -1) if k in ('wide_rows', 'poison') else int(x)
+    _check(_L.da4ml_cmvm_set_capacity_override(_ip(v)))
+    try:
+        yield
+    finally:
+        _L.da4ml_cmvm_set_capacity_override(None)
 
 
 def _fp(a):
@@ -276,7 +304,7 @@ class RawPipeline:
             self.launches = int(_L.da4ml_pipeline_launches(handle))
             prof = (C.c_double * 8)()
             _L.da4ml_pipeline_profile(handle, prof)
-            self.profile = dict(device_ms=prof[0], launches=int(prof[1]), solve_kernel_ms=prof[2], solve_kernel_launches=int(prof[3]), algo_bytes=prof[4], jobs_total=int(prof[5]), jobs_run=int(prof[6]))
+            self.profile = dict(device_ms=prof[0], launches=int(prof[1]), solve_kernel_ms=prof[2], solve_kernel_launches=int(prof[3]), algo_bytes=prof[4], jobs_total=int(prof[5]), jobs_run=int(prof[6]), solve_retries=int(prof[7]))
         finally:
             _L.da4ml_pipeline_free(handle)
 
@@ -479,7 +507,7 @@ class SweepResult:
         prof = (C.c_double * 8)()
         _check(_L.da4ml_sweep_profile(handle, prof))
         self.profile = dict(device_ms=prof[0], launches=int(prof[1]), solve_kernel_ms=prof[2], solve_kernel_launches=int(prof[3]), algo_bytes=prof[4],
-                            jobs_total=int(prof[5]), jobs_run=int(prof[6]), candidates=n, candidates_solved=self.n_solved, candidates_kept=self.n_kept)
+                            jobs_total=int(prof[5]), jobs_run=int(prof[6]), solve_retries=int(prof[7]), candidates=n, candidates_solved=self.n_solved, candidates_kept=self.n_kept)
 
     def __len__(self):
         return len(self.candidates['set'])

@@ -346,6 +346,21 @@ int da4ml_cmvm_set_accounting(int on) {
     g_accounting = on;
     return DA4ML_OK;
 }
+int da4ml_cmvm_set_capacity_override(const int64_t caps[8]) {
+    return guarded([&] {
+        int64_t v[CAP_KNOBS] = {-1, -1, -1, -1, -1, -1, -1, -1};
+        if (caps)
+            std::copy(caps, caps + CAP_KNOBS, v);
+        if (v[CAP_SEGMENT] == 0 || v[CAP_EXPR] == 0 || v[CAP_CELL_POOL] == 0)
+            throw ApiError(DA4ML_E_INVALID, "capacity override: segment_entries, expr_cap and cell_pool must be positive (or < 0 for the planner's)");
+        if (v[CAP_HASH_LOG] >= 0 && (v[CAP_HASH_LOG] < 8 || v[CAP_HASH_LOG] > 13))
+            throw ApiError(DA4ML_E_INVALID, "capacity override: hash_log must be in [8, 13] (or < 0 for the planner's)");
+        for (int64_t x : v)
+            if (x > (1LL << 30))
+                throw ApiError(DA4ML_E_INVALID, "capacity override: value out of range");
+        std::copy(v, v + CAP_KNOBS, g_cap_override);
+    });
+}
 
 int da4ml_cmvm_solve_batch(
     int64_t n_problems, const float *const *kernels, const int64_t *n_in, const int64_t *n_out, const char *method0,
@@ -457,6 +472,7 @@ int da4ml_cmvm_solve_single_seeded(
         pl->launches = tm.launches;
         pl->solve_ms = tm.solve_ms;
         pl->solve_launches = tm.solve_launches;
+        pl->solve_retries = tm.solve_retries;
         pl->algo_bytes = tm.algo_bytes;
         *out = new da4ml_pipeline();
         (*out)->impl = std::move(pl);
@@ -537,7 +553,7 @@ int da4ml_sweep_profile(const da4ml_sweep_t *s, double out[8]) {
     if (!s || !out)
         return DA4ML_E_INVALID;
     const PipelineImpl &t = s->impl->totals;
-    const double row[8] = {t.device_ms, (double)t.launches, t.solve_ms, (double)t.solve_launches, t.algo_bytes, (double)t.jobs_total, (double)t.jobs_run, 0.0};
+    const double row[8] = {t.device_ms, (double)t.launches, t.solve_ms, (double)t.solve_launches, t.algo_bytes, (double)t.jobs_total, (double)t.jobs_run, (double)t.solve_retries};
     std::copy(row, row + 8, out);
     return DA4ML_OK;
 }
@@ -908,7 +924,7 @@ int da4ml_pipeline_profile(const da4ml_pipeline_t *p, double out[8]) {
     out[4] = p->impl->algo_bytes;
     out[5] = (double)p->impl->jobs_total;
     out[6] = (double)p->impl->jobs_run;
-    out[7] = 0.0;
+    out[7] = (double)p->impl->solve_retries;
     return DA4ML_OK;
 }
 

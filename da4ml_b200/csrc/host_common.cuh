@@ -25,6 +25,11 @@ static cudaStream_t g_stream = nullptr;
 static int g_group_override = 0;
 static int g_accounting = 0;
 static int g_share_jobs = 1;  // solve byte-identical solve_single jobs of one call once (host_solve.cuh)
+// Test-only capacity squeeze (da4ml_cmvm_set_capacity_override), < 0 = the planner's value: histogram-segment entries
+// per CTA, shared-memory rows per owner list, spill rows per owner list, log2 of the pair-counter table, 12-byte list
+// rows, expression-table entries beyond the inputs, cells per CTA, 0xA5 in every buffer the driver does not clear.
+enum CapKnob { CAP_SEGMENT, CAP_LIST_ROWS, CAP_SPILL_ROWS, CAP_HASH_LOG, CAP_WIDE_ROWS, CAP_EXPR, CAP_CELL_POOL, CAP_POISON, CAP_KNOBS };
+static int64_t g_cap_override[CAP_KNOBS] = {-1, -1, -1, -1, -1, -1, -1, -1};
 
 struct ApiError : std::runtime_error {
     int code;
@@ -111,6 +116,7 @@ struct Timing {
     double solve_ms = 0;       // time inside cmvm_solve_kernel launches
     int64_t launches = 0;
     int64_t solve_launches = 0;
+    int64_t solve_retries = 0; // solve_single jobs relaunched after a capacity status
     double algo_bytes = 0;     // algorithmic bytes (SURVEY.md 8d) of every solve_single executed
     std::vector<std::pair<cudaEvent_t, cudaEvent_t>> pending;
     std::vector<char> is_solve;

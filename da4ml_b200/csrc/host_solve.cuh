@@ -16,7 +16,7 @@ namespace da {
 struct PipelineImpl {
     std::vector<StageResult> stages;
     double device_ms = 0, solve_ms = 0, algo_bytes = 0;
-    int64_t launches = 0, solve_launches = 0;
+    int64_t launches = 0, solve_launches = 0, solve_retries = 0;
     int64_t jobs_total = 0, jobs_run = 0; // solve_single jobs the reference would execute / executed after sharing identical ones
 };
 
@@ -551,6 +551,7 @@ static void solve_many(
         pl.launches = tm.launches;
         pl.solve_ms = tm.solve_ms;
         pl.solve_launches = tm.solve_launches;
+        pl.solve_retries = tm.solve_retries;
         pl.algo_bytes = tm.algo_bytes;
         pl.jobs_total = jobs_total;
         pl.jobs_run = jobs_run;

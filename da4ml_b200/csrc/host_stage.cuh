@@ -119,6 +119,41 @@ static int ilog2_ceil(int v) {
     return l;
 }
 
+// The test-only capacity squeeze (da4ml_cmvm_set_capacity_override) on a planned launch.  Each knob only lowers the
+// planner's value, and a retry raises it as it raises the planner's: the segment with f_mul, the spill rows and the cell
+// pool with list_mul / 2; the expression cap holds only until a job asks for the full table.  The workspace keeps the
+// planner's sizes; the spill rows also take the rows that shorter shared-memory lists give up.
+static void squeeze_plan(LaunchPlan &P, long long &seg_cap, const std::vector<StageJob *> &todo, std::vector<ProblemDesc> &desc, long long budget) {
+    const int64_t *ov = g_cap_override;
+    long long f_mul = 1, list_mul = 2;
+    for (const StageJob *j : todo) {
+        f_mul = std::max<long long>(f_mul, j->f_mul);
+        list_mul = std::max<long long>(list_mul, j->list_mul);
+    }
+    if (ov[CAP_SEGMENT] >= 0) // (no fewer than 4 pages)
+        seg_cap = std::min(P.max_fcap, std::max(ov[CAP_SEGMENT] * f_mul, 4LL << P.cfg.chunk_log));
+    if (ov[CAP_HASH_LOG] >= 0)
+        P.hlog = std::min<int>(P.hlog, (int)ov[CAP_HASH_LOG]);
+    long long lcap = P.lcap;
+    if (ov[CAP_LIST_ROWS] >= 0)
+        lcap = std::min<long long>(lcap, ov[CAP_LIST_ROWS]) & ~1LL;
+    if (ov[CAP_WIDE_ROWS] > 0 && P.narrow) { // twice the bytes per row: keep the rows that still fit the budget
+        P.narrow = 0;
+        const long long fixed = (long long)own_plan_bytes(P.cfg.nchunk_cap, P.n_out_max, P.e_cap_max, 0, P.hlog, 0);
+        lcap = std::min(lcap, std::max(0LL, (budget - fixed) / (12LL * P.n_out_max)) & ~1LL);
+    }
+    P.ovf_cap += P.lcap - lcap;
+    P.lcap = (int)lcap;
+    if (ov[CAP_SPILL_ROWS] >= 0)
+        P.ovf_cap = std::min(P.ovf_cap, ov[CAP_SPILL_ROWS] * list_mul / 2);
+    if (ov[CAP_CELL_POOL] >= 0)
+        P.pool_cap = std::min(P.pool_cap, ov[CAP_CELL_POOL] * list_mul / 2);
+    for (size_t i = 0; i < todo.size() && ov[CAP_EXPR] >= 0; ++i)
+        if (!todo[i]->full_expr)
+            desc[i].e_cap = (int)std::min<long long>(desc[i].e_cap, todo[i]->n_in + ov[CAP_EXPR]);
+    P.smem_bytes = own_plan_bytes(P.cfg.nchunk_cap, P.n_out_max, P.e_cap_max, P.lcap, P.hlog, P.narrow);
+}
+
 // Solve all jobs concurrently (one prep launch + one persistent solve launch per attempt).
 static void run_stage_jobs(std::vector<StageJob *> &jobs, Timing &tm, bool want_ops) {
     if (jobs.empty())
@@ -147,6 +182,9 @@ static void run_stage_jobs(std::vector<StageJob *> &jobs, Timing &tm, bool want_
         const size_t job_in_bytes = cj.off;
         g_job_arena.ensure(job_in_bytes, false);
         char *ja = (char *)g_job_arena.p;
+        const bool poison = g_cap_override[CAP_POISON] > 0;
+        if (poison)
+            CK(cudaMemsetAsync(ja, 0xA5, job_in_bytes, g_stream));
         // upload qint/lat through one pinned staging buffer
         {
             size_t up = 0;
@@ -247,6 +285,12 @@ static void run_stage_jobs(std::vector<StageJob *> &jobs, Timing &tm, bool want_
             d.op_q = (float4 *)g_out_arena2.take(sizeof(float4) * d.ops_cap);
             d.op_cost = (float *)g_out_arena2.take(sizeof(float) * d.ops_cap);
             d.out_q = (float4 *)g_out_arena2.take(sizeof(float4) * j.n_out);
+            if (poison) {
+                CK(cudaMemsetAsync(d.op_misc, 0xA5, sizeof(int4) * d.ops_cap, g_stream));
+                CK(cudaMemsetAsync(d.op_q, 0xA5, sizeof(float4) * d.ops_cap, g_stream));
+                CK(cudaMemsetAsync(d.op_cost, 0xA5, sizeof(float) * d.ops_cap, g_stream));
+                CK(cudaMemsetAsync(d.out_q, 0xA5, sizeof(float4) * j.n_out, g_stream));
+            }
             d.cost_init = j.cost_init;
             oo[i].oi = co.take(sizeof(int) * j.n_out);
             oo[i].os = co.take(sizeof(int) * j.n_out);
@@ -279,7 +323,11 @@ static void run_stage_jobs(std::vector<StageJob *> &jobs, Timing &tm, bool want_
         penv.accounting = accounting;
         penv.own_budget = g_own_smem_max - 1024;
         penv.group_override = g_group_override;
-        const LaunchPlan plan = plan_launch(pj, penv);
+        LaunchPlan plan = plan_launch(pj, penv);
+        const LaunchPlan planned = plan; // (the workspace sizes)
+        long long seg_cap = plan.max_fcap;
+        if (std::any_of(g_cap_override, g_cap_override + CAP_KNOBS, [](int64_t v) { return v >= 0; }))
+            squeeze_plan(plan, seg_cap, todo, desc, penv.own_budget);
         const LaunchCfg cfg = plan.cfg;
         const int G = cfg.G, n_groups = plan.n_groups;
         const long long max_fcap = plan.max_fcap;
@@ -291,6 +339,8 @@ static void run_stage_jobs(std::vector<StageJob *> &jobs, Timing &tm, bool want_
             throw ApiError(DA4ML_E_CAPACITY, "the solve kernel's shared-memory plan does not fit (" + std::to_string(smem_bytes) + " bytes)");
         static DevBuf g_out_arena;
         g_out_arena.ensure(co.off - job_in_bytes, false);
+        if (poison)
+            CK(cudaMemsetAsync(g_out_arena.p, 0xA5, co.off - job_in_bytes, g_stream));
         char *oa = (char *)g_out_arena.p - job_in_bytes;
         for (int i = 0; i < n; ++i) {
             ProblemDesc &d = desc[i];
@@ -316,13 +366,15 @@ static void run_stage_jobs(std::vector<StageJob *> &jobs, Timing &tm, bool want_
             wo[gi].heap = cw.take(sizeof(uint4) * 2 * max_heap);
             wo[gi].bar = cw.take(256);
             wo[gi].xchg = cw.take(sizeof(unsigned long long) * 2 * 4 * G);
-            wo[gi].e_col = cw.take(sizeof(uint32_t) * (size_t)G * plan.pool_cap);
-            wo[gi].e_pl0 = cw.take(sizeof(uint2) * (size_t)G * plan.pool_cap);
-            wo[gi].e_pl1 = cw.take(sizeof(uint2) * (size_t)G * plan.pool_cap);
+            wo[gi].e_col = cw.take(sizeof(uint32_t) * (size_t)G * planned.pool_cap);
+            wo[gi].e_pl0 = cw.take(sizeof(uint2) * (size_t)G * planned.pool_cap);
+            wo[gi].e_pl1 = cw.take(sizeof(uint2) * (size_t)G * planned.pool_cap);
             wo[gi].e_dir = cw.take(sizeof(uint2) * (size_t)max_ecap);
-            wo[gi].e_ovf = cw.take(sizeof(uint32_t) * 3 * (size_t)G * (size_t)max_cols * (size_t)std::max<long long>(plan.ovf_cap, 1));
+            wo[gi].e_ovf = cw.take(sizeof(uint32_t) * 3 * (size_t)G * (size_t)max_cols * (size_t)std::max<long long>({planned.ovf_cap, plan.ovf_cap, 1}));
         }
         g_ws_arena.ensure(cw.off, false);
+        if (poison)
+            CK(cudaMemsetAsync(g_ws_arena.p, 0xA5, cw.off, g_stream));
         std::vector<GroupWs> gws(n_groups);
         std::vector<OwnWs> ows(n_groups);
         char *wa = (char *)g_ws_arena.p;
@@ -336,7 +388,7 @@ static void run_stage_jobs(std::vector<StageJob *> &jobs, Timing &tm, bool want_
             w.fseg = (FEnt *)(wa + wo[gi].fseg);
             w.heap = (uint4 *)(wa + wo[gi].heap);
             w.barrier = (unsigned *)(wa + wo[gi].bar);
-            w.fseg_cap = (int)max_fcap;
+            w.fseg_cap = (int)seg_cap;
             w.heap_cap = max_heap;
             w.xchg = (unsigned long long *)(wa + wo[gi].xchg);
             CK(cudaMemsetAsync(w.barrier, 0, 256, g_stream));
@@ -521,6 +573,7 @@ static void run_stage_jobs(std::vector<StageJob *> &jobs, Timing &tm, bool want_
                 memcpy(j.trace, dp + dof[i].tr, sizeof(int) * 5 * (size_t)rows);
             }
         }
+        tm.solve_retries += (int64_t)again.size();
         todo.swap(again);
     }
     if (!todo.empty())

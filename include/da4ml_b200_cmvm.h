@@ -62,6 +62,16 @@ int da4ml_cmvm_set_accounting(int on);
  * pure function of its inputs, so by default identical jobs are solved once and the result shared (identical output to
  * the reference, which solves each candidate separately).  0 switches the sharing off. */
 int da4ml_cmvm_set_job_sharing(int on);
+/* Test-only capacity squeeze, so that small problems and the test suite reach the solve kernel's spill, multi-pass,
+ * compaction, overflow and retry paths on the device.  caps[8] (NULL resets; a value < 0 keeps the planner's) =
+ * {segment_entries (histogram entries per CTA, at least 4 pages), list_rows (shared-memory rows per owner list; 0 = every
+ * row spills), spill_rows (global-memory rows per owner list), hash_log (log2 of the pair-counter table, 8..13),
+ * wide_rows (> 0: 12-byte list rows), expr_cap (expression ids beyond the inputs), cell_pool (cells per CTA), poison
+ * (> 0: every buffer the driver does not clear is filled with 0xA5)}.  A value only lowers the planner's; the retry after
+ * a capacity status raises it as it raises the planner's (segment x f_mul, spill rows and cells x list_mul / 2; expr_cap
+ * is dropped with the full expression table), and the work buffers keep the planner's sizes.  All knobs < 0 (the
+ * default) leave every launch unchanged.  Results are unchanged too: a squeeze only makes the solver take longer paths. */
+int da4ml_cmvm_set_capacity_override(const int64_t caps[8]);
 
 /* ---- solve -------------------------------------------------------------------------------------
  * Replaces `solve` (bindings.cc:184-225 -> api.cc:147-250).
@@ -170,7 +180,7 @@ int da4ml_cmvm_solve_sweep_batch_seeded(
 /* counts: {n_sets, n_candidates, n_kept (candidates with op tables), n_solved (distinct candidates solved)} */
 int da4ml_sweep_counts(const da4ml_sweep_t *s, int64_t out[4]);
 /* Profile of the sweep call, as da4ml_pipeline_profile: {device_ms, launches, solve_kernel_ms, solve_kernel_launches,
- * algorithmic_bytes, jobs_total, jobs_run, 0}. */
+ * algorithmic_bytes, jobs_total, jobs_run, solve_retries}. */
 int da4ml_sweep_profile(const da4ml_sweep_t *s, double out[8]);
 /* Per candidate (either pointer may be NULL):
  *   ints   [n_candidates][12] int64 = {set, H, d (as started), method0, method1 (after api.cc:41-51 and any forced wmc-dc
@@ -210,7 +220,8 @@ double da4ml_pipeline_device_ms(const da4ml_pipeline_t *p);
 /* Number of kernel launches issued for the call that produced p. */
 int64_t da4ml_pipeline_launches(const da4ml_pipeline_t *p);
 /* Profile of the call that produced p: {device_ms, launches, solve_kernel_ms, solve_kernel_launches,
- * algorithmic_bytes (all solve_single jobs of the call, exact in accounting mode), 0, 0, 0}. */
+ * algorithmic_bytes (all solve_single jobs of the call, exact in accounting mode), jobs_total, jobs_run,
+ * solve_retries (solve_single jobs relaunched with larger capacities after a capacity status)}. */
 int da4ml_pipeline_profile(const da4ml_pipeline_t *p, double out[8]);
 
 /* ---- pipelined pricing ----------------------------------------------------------------------------
