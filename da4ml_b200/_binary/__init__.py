@@ -745,18 +745,22 @@ class ChainFront(NetworkFront):
     and jobs, in total and per layer (``layers[k]``: input-latency states, candidates, points kept, ...).
 
     ``activations``: the relu / quantizers between the layers that the front was searched with (``chain_front(...,
-    activations=...)``, each as ``(kind, [n_out, 3] kif)``), or ``None``.
+    activations=...)``, each as ``(kind, [n_out, 3] kif)``), or ``None``.  ``biases``: its per-layer biases (``None`` or
+    ``[n_out]`` float64 each), or ``None`` when it was searched without a non-zero one.
 
     Only host arrays are held (each point's designs are ``RawPipeline`` copies), so a front pickles as it is."""
 
     activations = None  # (a front built without activations holds no attribute of its own: it pickles as before)
+    biases = None  # (likewise without biases)
 
-    def __init__(self, cost, latency, choice, raws, calls, profile, latency_cutoff=0.0, activations=None):
+    def __init__(self, cost, latency, choice, raws, calls, profile, latency_cutoff=0.0, activations=None, biases=None):
         super().__init__(cost, latency, choice)
         self._raws, self._calls, self.profile = raws, calls, profile
         self.latency_cutoff = float(latency_cutoff)
         if activations is not None:
             self.activations = activations
+        if biases is not None:
+            self.biases = biases
         c = self.latency_cutoff
         # (to_pipeline's stage of the last output, + 1: the clock count of a chain whose network inputs arrive before c)
         self.stages = (np.floor(np.asarray(latency, np.float64) / (c + 1e-9)).astype(np.int64) + 1) if c > 0 else np.ones(len(cost), np.int64)
@@ -778,11 +782,17 @@ class ChainFront(NetworkFront):
         """Point ``p``'s designs as one ``Pipeline`` per layer."""
         return [r.to_pipeline(types_module) for r in self._raws[p]]
 
-    def design(self, p: int, activations=None) -> RawPipeline:
+    def design(self, p: int, activations=None, biases=None) -> RawPipeline:
         """Point ``p``'s designs as one chain design with ``activations`` between the layers: ``chain_design(self.pipelines(p),
-        activations)``, for ``price_pipelined`` (register bits, ``keep_split``).  A front searched with activations uses its
+        activations, biases)``, for ``price_pipelined`` (register bits, ``keep_split``).  A front searched with activations uses its
         own when none are given, and refuses others (``ValueError``): its later layers were solved for its own.  A front
-        searched without them needs them."""
+        searched without them needs them.  Biases likewise: the front's own are used, and other non-zero ones are refused."""
+        if biases is not None or self.biases is not None:
+            n_outs = [int(r.stages[-1]['shape'][1]) for r in self._raws[p]]
+            mine = self.biases or [None] * len(n_outs)
+            theirs = mine if biases is None else (_biases_arg(biases, n_outs) or [None] * len(n_outs))
+            if any((a is None) != (b is None) or (a is not None and not np.array_equal(a, b)) for a, b in zip(mine, theirs)):
+                raise ValueError('these biases differ from the ones the front was searched with: its later layers were solved for those')
         if activations is None:
             if self.activations is None:
                 raise TypeError('this front was searched without activations: design(p, activations) needs them')
@@ -795,7 +805,7 @@ class ChainFront(NetworkFront):
                 same &= a_kind == kind and np.array_equal(a_kif, kif)
             if not same:
                 raise ValueError('these activations differ from the ones the front was searched with: its later layers were solved for those')
-        return chain_design(self._raws[p], activations)
+        return chain_design(self._raws[p], activations, self.biases)
 
     def reference_calls(self, p: int) -> list[dict]:
         """Per layer, the keywords of the ``solve(kernels[k], **kw)`` call that returns layer ``k``'s design in point
@@ -818,12 +828,13 @@ def _chain_layer(points, state_of, sweeps, state_lats, traced=None, state_qs=Non
     solver's; a front candidate without an entry is dropped.
 
     Chains with activations: ``state_qs[s]`` are state ``s``'s qintervals for the reference calls, and ``acted`` is
-    ``(group_of, table)`` at every layer but the last: ``group_of[p]`` is parent ``p``'s replay group (the parents of one state with the same float64
+    ``(group_of, table, ...)`` at every layer but the last (and at the last when it has a bias): ``group_of[p]`` is parent ``p``'s replay group (the parents of one state with the same float64
     input intervals); ``table[g, i]`` is ``None`` when candidate ``i`` under group ``g`` makes a non-zero constant (the
-    pair is dropped), else ``(act_cost, zero, intervals)``: the float32 cost of each output's activation op (0 without
-    one), which outputs become the constant 0, and the outputs' intervals after the activation.  A point's cost then
-    continues with ``act_cost`` added in output order, and its ``outs`` entry is ``(latencies, intervals)``, the latency
-    of a constant 0 being 0."""
+    pair is dropped), else ``(act_cost, zero, intervals, views)``: the float32 cost of each op of the bias / activation
+    stage in stage order (with a bias: each output's constant addition, then each output's activation op; 0 without
+    one), which outputs become the constant 0, the outputs' intervals after the bias and activation, and their
+    ``[n, 2]`` (factor, cadd) of ``_traced_views``.  A point's cost then continues with ``act_cost`` added in order, and
+    its ``outs`` entry is ``(latencies, intervals, views)``, the latency of a constant 0 being 0."""
     fronts = [np.asarray(sw.front, np.int64) for sw in sweeps]
     if traced is not None:
         fronts = [np.asarray([i for i in f.tolist() if (s, i) in traced], np.int64) for s, f in enumerate(fronts)]
@@ -838,7 +849,7 @@ def _chain_layer(points, state_of, sweeps, state_lats, traced=None, state_qs=Non
     cost = np.concatenate([f_cost[s] for s in state_of])
     lat = np.concatenate([f_lat[s] for s in state_of])
     if acted is not None:
-        group_of, table = acted
+        group_of, table = acted[:2]
         ok = np.asarray([table[group_of[p], i] is not None for p, i in zip(par.tolist(), cand.tolist())], bool).reshape(-1)
         par, sidx, cand, cost, lat = par[ok], sidx[ok], cand[ok], cost[ok], lat[ok]
     if points is not None:
@@ -863,14 +874,14 @@ def _chain_layer(points, state_of, sweeps, state_lats, traced=None, state_qs=Non
         raws.append([r] if points is None else [*points[4][p], r])
         calls.append([call] if points is None else [*points[5][p], call])
         if acted is not None:
-            _, zero, vals = table[group_of[p], i]
-            o = (np.where(zero, 0.0, o).astype(o.dtype), vals)
+            _, zero, vals, aux = table[group_of[p], i]
+            o = (np.where(zero, 0.0, o).astype(o.dtype), vals, aux)
         outs.append(o)
     return cost, lat, choice, outs, raws, calls
 
 
 def chain_front(kernels, option_sets, qintervals=None, latencies=None, adder_size=-1, carry_size=-1, solver=None, latency_cutoff=0.0, pricer=None,
-                activations=None) -> ChainFront:
+                activations=None, biases=None) -> ChainFront:
     """The cost / latency front of a chain of layers, each layer solved under the output latencies of the design chosen
     for the layer before it, as a traced model's matmuls are: every reported design is what
     ``solve(kernels[k], **front.reference_calls(p)[k])`` returns, and every reported cost and latency is the chain's own.
@@ -916,9 +927,20 @@ def chain_front(kernels, option_sets, qintervals=None, latencies=None, adder_siz
     chains on (cost, latency) is a heuristic and a pruned chain could have led to a better design.  What is reported is
     exact.
 
+    ``biases`` (needs ``activations``; ``None``, or one per layer: ``None`` or an ``[n_out_k]`` array) are added to each
+    layer's outputs before its activation, in ``chain_design``'s format; the last layer's bias is allowed.  The search
+    states are then the (latencies, intervals) after bias and activation, and a point's cost is the float32 sum in stage
+    order of ``design(p)``'s cost column, its bias / activation stage's ops in the order: input ops (cost 0), each
+    output's constant addition, each output's activation op.  A pair whose bias makes a non-zero constant is dropped
+    (``dropped_constant``), and one whose bias the tracer folds into the previous layer's (``chain_design``'s folding case)
+    is dropped and counted in ``profile['layers'][k]['dropped_folded']``, and one whose bias op is not exact in the stage
+    arrays (float32 intervals, ``|data| < 2**31``; ``chain_design`` refuses it) in ``dropped_inexact``.  The bias values
+    themselves are checked before any device call.  ``biases=None`` and all-zero biases give the front without them.
+
     Limits: a layer's states all run in one call, and their op tables stay on the device until that call ends; if they do
     not fit (``DA4ML_E_CAPACITY``), or any set fails on any state, the call raises that layer's error prefixed with
-    ``layer k: `` and returns nothing.  Branching networks are not covered.  ``solver(kernels, option_sets, **kw)`` stands
+    ``layer k: `` and returns nothing.  Branching networks are not covered, nor is a bias the tracer folds across an
+    activation (above).  ``solver(kernels, option_sets, **kw)`` stands
     in for ``solve_sweep_batch`` (same keywords and results), ``pricer`` for ``price_pipelined``."""
     ks = [_prefixed(f'layer {k}', _kernel_arg, W) for k, W in enumerate(kernels)]
     if not ks:
@@ -938,6 +960,11 @@ def chain_front(kernels, option_sets, qintervals=None, latencies=None, adder_siz
         for k in range(1, len(ks) if qintervals is not None else 0):
             if qintervals[k] is not None:
                 raise ValueError(f"layer {k}: with activations a layer's qintervals are its traced inputs' (only layer 0's may be given)")
+    bs = None
+    if biases is not None:
+        if acts is None:
+            raise ValueError('biases need activations (an empty list for one layer): a chain with biases is solved under its traced intervals')
+        bs = _biases_arg(biases, [int(W.shape[1]) for W in ks])
     qs = [None if qintervals is None else _prefixed(f'layer {k}', _qint_arg, qintervals[k], W.shape[0]) for k, W in enumerate(ks)]
     qs = [None if q is None else [tuple(map(float, r)) for r in q] for q in qs]
     l0 = _prefixed('layer 0', _lat_arg, latencies, ks[0].shape[0])
@@ -958,12 +985,12 @@ def chain_front(kernels, option_sets, qintervals=None, latencies=None, adder_siz
             states = [np.frombuffer(b, dt) for b in index]
         elif k > 0:  # one state per distinct (output latencies, float32 activated intervals), in order of first use
             index, first = {}, []
-            for p, (o, v) in enumerate(points[3]):
+            for p, (o, v, *_) in enumerate(points[3]):
                 key = np.asarray(o, dt).tobytes() + np.asarray(v, np.float32).tobytes()
                 if key not in index:
                     index[key] = len(first)
                     first.append(p)
-            state_of = np.asarray([index[np.asarray(o, dt).tobytes() + np.asarray(v, np.float32).tobytes()] for o, v in points[3]], np.int64)
+            state_of = np.asarray([index[np.asarray(o, dt).tobytes() + np.asarray(v, np.float32).tobytes()] for o, v, *_ in points[3]], np.int64)
             states = [np.asarray(points[3][p][0], dt) for p in first]
             state_qs = [[tuple(map(float, r)) for r in np.asarray(points[3][p][1], np.float32)] for p in first]
         n, lats = len(states), [[float(v) for v in s] for s in states]
@@ -976,16 +1003,20 @@ def chain_front(kernels, option_sets, qintervals=None, latencies=None, adder_siz
             traced = {key: (float(pr.latency_max[j, 0]), np.asarray(pr.out_latency(j, 0), np.float64)) for j, key in enumerate(keys) if int(pr.status[j, 0]) == 0}
             priced = dict(dropped=len(keys) - len(traced), price_launches=int(pr.profile.get('launches', 0)), price_device_ms=float(pr.profile.get('device_ms', 0.0)))
         acted, replayed = None, {}
-        if acts is not None and k < len(ks) - 1:
+        bias = None if bs is None else bs[k]
+        if acts is not None and (k < len(ks) - 1 or bias is not None):
             t0 = time.perf_counter()
-            acted = _chain_replay(points, state_of, sweeps, traced, k, *acts[k])
-            replayed = dict(replay_ms=(time.perf_counter() - t0) * 1e3, dropped_constant=sum(v is None for v in acted[1].values()))
+            acted = _chain_replay(points, state_of, sweeps, traced, k, *(acts[k] if k < len(acts) else (None, None)), bias)
+            replayed = dict(replay_ms=(time.perf_counter() - t0) * 1e3, dropped_constant=acted[2]['constant'])
+            if bs is not None:
+                replayed.update(dropped_folded=acted[2]['folded'], dropped_inexact=acted[2]['inexact'])
         elif acts is not None:
-            replayed = dict(replay_ms=0.0, dropped_constant=0)
+            replayed = dict(replay_ms=0.0, dropped_constant=0, **({} if bs is None else dict(dropped_folded=0, dropped_inexact=0)))
         points = _chain_layer(points, state_of, sweeps, lats, traced, None if acts is None else state_qs, acted)
         if len(points[0]) == 0:
-            if replayed.get('dropped_constant'):
-                raise ValueError(f'layer {k}: every front candidate is slower than the latency cutoff {c} or makes an output of activation {k} a non-zero constant')
+            if replayed.get('dropped_constant') or replayed.get('dropped_folded') or replayed.get('dropped_inexact'):
+                raise ValueError(f'layer {k}: every front candidate is slower than the latency cutoff {c}, makes an output of bias / activation {k} a '
+                                 'non-zero constant, has a bias the tracer folds or a bias op that is not exact in the stage arrays')
             raise ValueError(f'layer {k}: every front candidate has an adder slower than the latency cutoff {c}')
         p0 = sweeps[0].profile  # (the whole call's)
         layer = dict(states=n, candidates=sum(len(sw.candidates['cost']) for sw in sweeps), points=len(points[0]),
@@ -996,37 +1027,56 @@ def chain_front(kernels, option_sets, qintervals=None, latencies=None, adder_siz
         del sweeps  # (the designs are copied out: free the handles before the next layer's call)
     cost, lat, choice, _, raws, calls = points
     order = np.argsort(lat, kind='stable')
-    return ChainFront(cost[order], lat[order], choice[order], [raws[p] for p in order], [calls[p] for p in order], prof, c, acts)
+    return ChainFront(cost[order], lat[order], choice[order], [raws[p] for p in order], [calls[p] for p in order], prof, c, acts, bs)
 
 
 _ZERO_QINT = (0.0, 0.0, 2.0**32)  # the tracer's constant 0: FixedVariable gives a constant the step 2**-_const_f(0) = 2**32
 
 
-def _chain_replay(points, state_of, sweeps, traced, k, kind, kif):
+def _chain_replay(points, state_of, sweeps, traced, k, kind, kif, bias=None):
     """``_chain_layer``'s ``acted`` for layer ``k`` of a chain with activations: every front candidate (that pricing
-    kept) of every state, replayed through activation ``k`` from each distinct float64 input intervals of the state's
-    parents (at layer 0, the design's own input intervals, as in ``chain_design``)."""
-    group_of, groups = [], {}  # parent -> replay group; (state, float64 intervals) -> group
+    kept) of every state, replayed through bias ``k`` and activation ``k`` (``kind`` ``None``: the last layer's bias alone)
+    from each distinct float64 input values of the state's parents (at layer 0, the design's own input intervals, as in
+    ``chain_design``).  A table entry is ``None`` for a dropped pair; its reason goes to the returned counts
+    (``constant``, ``folded``, ``inexact``)."""
+    group_of, groups = [], {}  # parent -> replay group; (state, float64 intervals and views) -> group
     for p, s in enumerate(state_of.tolist()):
-        vin = None if points is None else np.asarray(points[3][p][1], np.float64)
-        group_of.append(groups.setdefault((s, None if vin is None else vin.tobytes()), len(groups)))
-    table = {}
-    for (s, vb), g in groups.items():
+        key = None if points is None else np.asarray(points[3][p][1], np.float64).tobytes() + np.asarray(points[3][p][2], np.float64).tobytes()
+        group_of.append(groups.setdefault((s, key), len(groups)))
+    table, drops = {}, dict(constant=0, folded=0, inexact=0)
+    for (s, key), g in groups.items():
         for i in np.asarray(sweeps[s].front, np.int64).tolist():
             if traced is not None and (s, i) not in traced:
                 continue
             stages = sweeps[s].raw(i).stages
-            vals = _input_intervals(stages) if vb is None else [tuple(r) for r in np.frombuffer(vb, np.float64).reshape(-1, 3).tolist()]
+            if key is None:
+                vals = _input_intervals(stages)
+            else:
+                q = np.frombuffer(key, np.float64)
+                n = q.size // 5
+                vals = [(*r[:3], r[3], bool(r[4])) for r in np.concatenate([q[: 3 * n].reshape(n, 3), q[3 * n :].reshape(n, 2)], axis=1).tolist()]
             try:
-                traced_vals, changed = _activated_intervals(stages, vals, k, kind, kif)
+                traced_vals, biased, changed, nxt = _activated_intervals(stages, vals, k, kind, kif, bias)
+            except _FoldedBias:
+                table[g, i] = None
+                drops['folded'] += 1
+                continue
+            except _InexactBias:
+                table[g, i] = None
+                drops['inexact'] += 1
+                continue
             except _ConstantValue:
                 table[g, i] = None
+                drops['constant'] += 1
                 continue
             act_cost = np.asarray([0.0 if a is None else a[3] for a in changed], np.float32)
-            zero = np.asarray([a is not None and a[0] == a[1] for a in changed], bool)
-            vals = [t if a is None else _ZERO_QINT if a[0] == a[1] else a[:3] for t, a in zip(traced_vals, changed)]
-            table[g, i] = (act_cost, zero, np.asarray(vals, np.float64).reshape(-1, 3))
-    return group_of, table
+            if bias is not None:  # (stage order: the constant additions, then the activation ops)
+                act_cost = np.concatenate([np.asarray([0.0 if c is None else c[3] for c in biased], np.float32), act_cost])
+            zero = np.asarray([v[0] == v[1] for v in nxt], bool)
+            vals = [_ZERO_QINT if v[0] == v[1] else v[:3] for v in nxt]
+            aux = np.asarray([v[3:] for v in nxt], np.float64).reshape(-1, 2)
+            table[g, i] = (act_cost, zero, np.asarray(vals, np.float64).reshape(-1, 3), aux)
+    return group_of, table, drops
 
 
 def _kif_prop(lo: float, hi: float, step: float) -> tuple[int, int, int]:
@@ -1066,35 +1116,107 @@ def _activate(kind: str, lo: float, hi: float, step: float, k: int, i: int, f: i
     return l, h, st
 
 
-def _traced_intervals(stages, vals):
-    """The intervals (lo, hi, step) of a design's outputs as the tracer's replay (``CombLogic.__call__`` on
-    ``FixedVariable``s) gives them for inputs of intervals ``vals``: sums of the operands' scaled intervals, which can be
-    wider than the ones the solver records.  A dead column is the constant 0, (0, 0, 1)."""
+def _traced_views(stages, vals):
+    """``_traced_intervals`` with each output's factor and kind: (lo, hi, step, factor, cadd) per output, ``factor`` the
+    +-2**k of the tracer's view of it (``FixedVariable._factor``: the operand with a positive factor leads an addition,
+    shifts and negations scale it) and ``cadd`` whether that view is of a constant addition (``opr == 'cadd'``, which
+    ``_pow2_mul``, ``__neg__`` and an addition of the constant 0 keep).  ``vals`` entries are (lo, hi, step) (factor 1, not
+    a constant addition) or such 5-tuples."""
+    vals = [tuple(v) if len(v) == 5 else (*v, 1.0, False) for v in vals]
     for st in stages:
-        ins = [(lo * 2.0**sh, hi * 2.0**sh, s * 2.0**sh) for (lo, hi, s), sh in zip(vals, np.asarray(st['inp_shifts'], np.int64).tolist())]
+        ins = [(lo * 2.0**sh, hi * 2.0**sh, s * 2.0**sh, f * 2.0**sh, c) for (lo, hi, s, f, c), sh in zip(vals, np.asarray(st['inp_shifts'], np.int64).tolist())]
         buf = []
         for id0, id1, opc, data in np.asarray(st['ops_i'], np.int64).reshape(-1, 4).tolist():
             if opc == -1:
                 buf.append(ins[id0])
                 continue
-            a, (lo, hi, s) = buf[id0], buf[id1]
-            b = (lo * 2.0**data, hi * 2.0**data, s * 2.0**data)
+            a, (lo, hi, s, f, c) = buf[id0], buf[id1]
+            b = (lo * 2.0**data, hi * 2.0**data, s * 2.0**data, f * 2.0**data, c)
             if opc == 1:
-                b = (-b[1], -b[0], b[2])
-            buf.append((a[0] + b[0], a[1] + b[1], min(a[2], b[2])) if a[0] != a[1] and b[0] != b[1] else (b if a[0] == a[1] else a))
+                b = (-b[1], -b[0], b[2], -b[3], c)
+            if a[0] != a[1] and b[0] != b[1]:
+                buf.append((a[0] + b[0], a[1] + b[1], min(a[2], b[2]), a[3] if a[3] > 0 or b[3] < 0 else b[3], False))
+            else:
+                buf.append(b if a[0] == a[1] else a)
         vals = []
         for i, sh, ng in zip(np.asarray(st['out_idxs'], np.int64).tolist(), np.asarray(st['out_shifts'], np.int64).tolist(), np.asarray(st['out_negs']).astype(bool).tolist()):
             if i < 0:
-                vals.append((0.0, 0.0, 1.0))
+                vals.append((0.0, 0.0, 1.0, 1.0, False))
                 continue
-            lo, hi, s = (v * 2.0**sh for v in buf[i])
-            vals.append((-hi, -lo, s) if ng else (lo, hi, s))
+            lo, hi, s, f = (v * 2.0**sh for v in buf[i][:4])
+            vals.append((-hi, -lo, s, -f, buf[i][4]) if ng else (lo, hi, s, f, buf[i][4]))
     return vals
+
+
+def _traced_intervals(stages, vals):
+    """The intervals (lo, hi, step) of a design's outputs as the tracer's replay (``CombLogic.__call__`` on
+    ``FixedVariable``s) gives them for inputs of intervals ``vals``: sums of the operands' scaled intervals, which can be
+    wider than the ones the solver records.  A dead column is the constant 0, (0, 0, 1)."""
+    return [v[:3] for v in _traced_views(stages, vals)]
+
+
+def _const_f(c: float) -> int:
+    """``_const_f`` of the tracer (trace/fixed_variable.py:201-214): the least f in (-32, 32] with ``c * 2**f`` an integer."""
+    if c == 0:
+        return -32
+    lo, hi = -32, 32
+    while hi - lo > 1:
+        mid = (hi + lo) // 2
+        v = c * 2.0**mid
+        if v == int(v):
+            hi = mid
+        else:
+            lo = mid
+    return hi
+
+
+def _exact_sum(a: float, b: float) -> float | None:
+    """``a + b`` when it is exact in float64 (the tracer adds Decimals), else ``None``."""
+    s = a + b
+    bb = s - a
+    return s if (a - (s - bb)) + (b - bb) == 0.0 else None
+
+
+def _bias_op(j: int, k: int, v, b: float):
+    """What the tracer's ``v + b`` (``FixedVariable._const_add``, trace/fixed_variable.py:484-513) makes of output ``j`` of
+    layer ``k``, ``v`` its (lo, hi, step, factor, cadd) and ``b`` a non-zero bias: (lo, hi, step, cost, data) of the
+    constant-addition node in the value's own units, ``data`` the bias in steps of the result.  Its cost is the tracer's,
+    ``ceil(log2(|b / factor| + 2**-f)) + f`` with ``f = _const_f(b / factor)``.  ``_ConstantValue`` for a constant
+    result; ``_FoldedBias`` when ``v`` is itself a constant addition (the tracer folds the two); ``ValueError`` when the op
+    is not exact in the stage arrays (float32 intervals, an int32 ``data``): ``_InexactBias``."""
+    from fractions import Fraction
+    from math import ceil, log2
+
+    lo, hi, st, fac, cadd = v
+    if lo == hi:
+        raise _ConstantValue(f'bias {k}: output {j} of layer {k} is the constant {_exact_sum(lo, b)} (only the constant 0 is covered)')
+    if cadd:
+        raise _FoldedBias(f'bias {k}: output {j} of layer {k} passes a biased value of the layer before through unchanged, and the tracer folds '
+                          'the two biases into one constant addition across the activation (not covered)')
+    l, h = _exact_sum(lo, b), _exact_sum(hi, b)
+    step = min(st, 2.0 ** -_const_f(b))
+    data = b / step
+    if l is None or h is None or any(float(np.float32(x)) != x for x in (l, h, step)) or abs(data) >= 2**31:
+        raise _InexactBias(f'bias {k}: output {j} of layer {k} plus {b!r} is not exact in the stage arrays (float32 intervals, |bias / step| < 2**31)')
+    d = b / fac
+    f = _const_f(d)
+    cost = float(ceil(log2(float(abs(Fraction(d)) + Fraction(2) ** -f))) + f)
+    return l, h, step, cost, int(data)
 
 
 class _ConstantValue(ValueError):
     """A value of a chain that is or becomes a constant other than 0: ``chain_design`` refuses it, ``chain_front`` drops
     the candidate."""
+
+
+class _InexactBias(ValueError):
+    """A bias whose constant addition is not exact in the stage arrays (float32 intervals, ``|data| < 2**31``):
+    ``chain_design`` refuses it, ``chain_front`` drops the candidate."""
+
+
+class _FoldedBias(ValueError):
+    """A bias the tracer folds into the constant addition of the layer before (a pass-through column of a biased value
+    that the activation left unchanged): ``chain_design`` refuses it, ``chain_front`` drops the candidate."""
 
 
 def _input_intervals(stages) -> list:
@@ -1107,32 +1229,77 @@ def _input_intervals(stages) -> list:
     return vals
 
 
-def _activated_intervals(stages, vals, k: int, kind: str, kif):
-    """One step of the tracer's interval replay of a chain: layer ``k``'s design (``stages``) on inputs of intervals
-    ``vals`` (``_traced_intervals``), then activation ``k`` (``kind``, ``[n_out, 3]`` kif) on every output.  Returns
-    ``(traced, acts)``: ``traced[j]`` is output ``j``'s (lo, hi, step); ``acts[j]`` is ``None`` when the activation leaves it
-    unchanged, else the (lo, hi, step, cost) of the op the tracer records for it (cost ``sum(kif) / 2`` for relu, 0 for
-    quantize), or (0.0, 0.0, 1.0, 0.0) for the constant 0 (a dead column, or a format with no bits left).
-    ``_ConstantValue`` when a value is or becomes any other constant.  The one Python copy of these rules (the C++ copy
-    is ``pp_prepare``'s)."""
-    traced = _traced_intervals(stages, vals)
-    acts = []
-    for j, (lo, hi, st) in enumerate(traced):
+def _activated_intervals(stages, vals, k: int, kind, kif, bias=None):
+    """One step of the tracer's interval replay of a chain: layer ``k``'s design (``stages``) on inputs ``vals``
+    (``_traced_views``), then bias ``k`` (``None`` or ``[n_out]`` float64, added to every output with
+    ``FixedVariable._const_add``), then activation ``k`` (``kind``, ``[n_out, 3]`` kif; ``kind`` ``None``: none, as after
+    the last layer) on every output.  Returns ``(traced, biased, acts, nxt)``: ``traced[j]`` is output ``j``'s (lo, hi,
+    step); ``biased[j]`` is ``None`` without a bias op, else the (lo, hi, step, cost, data) of the constant addition the
+    tracer records (``_bias_op``); ``acts[j]`` is ``None`` when the activation leaves the (biased) value unchanged, else
+    the (lo, hi, step, cost) of the op the tracer records for it (cost ``sum(kif) / 2`` for relu, 0 for quantize), or (0.0,
+    0.0, 1.0, 0.0) for the constant 0 (a dead column, or a format with no bits left); ``nxt[j]`` is the value handed on,
+    as (lo, hi, step, factor, cadd).  ``_ConstantValue`` when a value is or becomes any other constant, ``_FoldedBias``
+    for a bias the tracer folds.  The one Python copy of these rules (the C++ copy is ``pp_prepare``'s)."""
+    views = _traced_views(stages, vals)
+    traced = [v[:3] for v in views]
+    biased, acts, nxt = [], [], []
+    for j, v in enumerate(views):
+        b = 0.0 if bias is None else float(bias[j])
+        if b != 0.0:
+            r = _bias_op(j, k, v, b)
+            biased.append(r)
+            v = (*r[:3], v[3], True)
+        else:
+            biased.append(None)
+        lo, hi, st = v[:3]
         if lo == hi:
             if lo != 0.0 or hi != 0.0:
                 raise _ConstantValue(f'activation {k}: output {j} of layer {k} is the constant {lo} (only the constant 0 is covered)')
-            acts.append((0.0, 0.0, 1.0, 0.0))
+            acts.append(None if kind is None else (0.0, 0.0, 1.0, 0.0))
+            nxt.append((0.0, 0.0, 1.0, 1.0, False))
             continue
-        r = _activate(kind, lo, hi, st, *(int(v) for v in kif[j]))
+        r = None if kind is None else _activate(kind, lo, hi, st, *(int(x) for x in kif[j]))
         if r is None:
             acts.append(None)
+            nxt.append(v)
         elif r[0] == r[1]:
             if r[0] != 0.0:
                 raise _ConstantValue(f'activation {k}: output {j} becomes the constant {r[0]} (only the constant 0 is covered)')
             acts.append((0.0, 0.0, 1.0, 0.0))
+            nxt.append((0.0, 0.0, 1.0, 1.0, False))
         else:
             acts.append((*r, sum(_kif_prop(*r)) / 2 if kind == 'relu' else 0.0))
-    return traced, acts
+            nxt.append((*r, abs(v[3]), False))
+    return traced, biased, acts, nxt
+
+
+def _bias_arg(k: int, b, n: int):
+    """``None`` (no bias, or an all-zero one) or the ``[n]`` float64 bias ``k`` of ``chain_design`` / ``chain_front``."""
+    if b is None:
+        return None
+    try:
+        a = np.asarray(b, np.float64)
+    except (TypeError, ValueError):
+        raise ValueError(f'bias {k}: expected None or {n} numbers, got {b!r}') from None
+    if a.shape != (n,):
+        raise ValueError(f'bias {k}: expected None or shape ({n},), got shape {a.shape}')
+    if not np.isfinite(a).all():
+        raise ValueError(f'bias {k}: every value must be finite')
+    sc = a * 2.0**32
+    if not (np.abs(sc) < 2.0**63).all() or (sc != np.round(sc)).any():
+        raise ValueError(f'bias {k}: every value must be a multiple of 2**-32 (the tracer finds a constant\'s step in [2**-32, 2**32]), with |value| < 2**31')
+    return a if (a != 0).any() else None
+
+
+def _biases_arg(biases, n_outs):
+    """Per layer ``None`` or its ``[n_out]`` bias (``_bias_arg``), or ``None`` when no layer has a non-zero one."""
+    if biases is None:
+        return None
+    bs = list(biases)
+    if len(bs) != len(n_outs):
+        raise ValueError(f'{len(n_outs)} layers need {len(n_outs)} biases (None for none), got {len(bs)}')
+    bs = [_bias_arg(k, b, n) for k, (b, n) in enumerate(zip(bs, n_outs))]
+    return bs if any(b is not None for b in bs) else None
 
 
 def _act_arg(k: int, act, n: int):
@@ -1163,7 +1330,7 @@ def _act_arg(k: int, act, n: int):
     return kind, a
 
 
-def chain_design(designs, activations) -> RawPipeline:
+def chain_design(designs, activations, biases=None) -> RawPipeline:
     """A chain of solver designs with a relu or quantizer between consecutive layers, as ONE design: layer 0's stages, an
     activation stage, layer 1's stages, and so on.  ``price_pipelined`` prices and splits it as the reference's tracer
     pipelines the whole model: ``to_pipeline(comb_trace(inp, chain(inp)), c, retiming)``, where ``chain`` replays every
@@ -1185,7 +1352,20 @@ def chain_design(designs, activations) -> RawPipeline:
     inputs arrived at 0, and ``price_pipelined`` re-traces every latency anyway.  A value the tracer passes through unchanged (``quantize`` to a
     wider format, ``relu`` of a non-negative value) gets no op: its output reads the input op.  A value that becomes the
     constant 0 (a dead column, or a format with no bits left) is a dead output column (``out_idx -1``).  A value that would
-    become any other constant is refused with ``ValueError``.  All checks run on the host, before any device call."""
+    become any other constant is refused with ``ValueError``.
+
+    ``biases[k]`` (``None``, or one per layer: ``None`` or an ``[n_out_k]`` array) is added to layer ``k``'s outputs before
+    activation ``k``, as ``x @ W_k + b_k`` adds it in a traced model (``FixedVariable._const_add``).  A non-zero bias gets
+    the op the tracer records, in the activation stage between the input ops and the activation ops: opcode 4 reading the
+    value's input op, ``data`` the bias in steps of the result, the interval ``(lo + b, hi + b)`` with step ``min(step,
+    2**-_const_f(b))`` and the tracer's cost ``ceil(log2(|b / factor| + 2**-f)) + f`` (``f = _const_f(b / factor)``,
+    ``factor`` the sign and scaling of the tracer's view of the value); the activation op of that value reads it.  A zero
+    bias records nothing, so all-zero biases give the design without them.  The last layer's bias gets a trailing stage of
+    its own, with no activation.  A bias is refused (``ValueError``) when it is not finite or not a multiple of 2**-32,
+    when its op is not exact in the stage arrays (float32 intervals, ``|data| < 2**31``), when it makes a non-zero
+    constant (a bias on a dead column or on a value the activation zeroed), and when the tracer would fold it into the
+    bias of the layer before (a column that passes a biased value through unchanged: the folded op would read a node on
+    the far side of the activation stage).  All checks run on the host, before any device call."""
     stages = [_design_stages(d) for d in designs]
     if not stages:
         raise ValueError('chain_design needs at least one design')
@@ -1199,33 +1379,57 @@ def chain_design(designs, activations) -> RawPipeline:
     for k in range(1, len(stages)):
         if stages[k - 1][-1]['shape'][1] != stages[k][0]['shape'][0]:
             raise ValueError(f"layer {k - 1} has {stages[k - 1][-1]['shape'][1]} outputs but layer {k} has {stages[k][0]['shape'][0]} inputs")
-    kinds = [_act_arg(k, act, int(stages[k][-1]['shape'][1])) for k, act in enumerate(acts)]
+    n_outs = [int(st[-1]['shape'][1]) for st in stages]
+    kinds = [_act_arg(k, act, n_outs[k]) for k, act in enumerate(acts)]
+    bs = _biases_arg(biases, n_outs)
     vals = _input_intervals(stages[0])
     out = [dict(st) for st in stages[0]]
-    for k, (kind, kif) in enumerate(kinds):
-        last = stages[k][-1]
-        n = int(last['shape'][1])
-        traced, changed = _activated_intervals(stages[k], vals, k, kind, kif)
-        idx = np.asarray(last['out_idxs'], np.int64)
-        of = np.asarray(last['ops_f'], np.float64).reshape(-1, 5)
-        ops_i, ops_f, out_idxs = [], [], np.zeros(n, np.int64)
-        for j in range(n):  # the input ops first, in value order: the traced interval and the solver's latency
-            ops_i.append([j, -1, -1, 0])
-            ops_f.append([*traced[j], float(of[idx[j], 3]) if idx[j] >= 0 else 0.0, 0.0])
-        for j, a in enumerate(changed):
-            if a is None:
-                out_idxs[j] = j
-            elif a[0] == a[1]:  # (the constant 0)
-                out_idxs[j] = -1
-            else:
-                out_idxs[j] = len(ops_i)
-                ops_i.append([j, -1, 2 if kind == 'relu' else 3, 0])
-                ops_f.append([*a[:3], ops_f[j][3], a[3]])
-        vals = [tuple(ops_f[i][:3]) if i >= 0 else (0.0, 0.0, 1.0) for i in out_idxs.tolist()]
-        out.append(dict(shape=(n, n), inp_shifts=np.zeros(n, np.int64), out_idxs=out_idxs, out_shifts=np.zeros(n, np.int64), out_negs=np.zeros(n, np.int64),
-                        ops_i=np.asarray(ops_i, np.int64).reshape(-1, 4), ops_f=np.asarray(ops_f, np.float32).reshape(-1, 5), adder_size=a_sz, carry_size=c_sz))
-        out += [dict(st) for st in stages[k + 1]]
+    for k in range(len(stages)):
+        kind, kif = kinds[k] if k < len(kinds) else (None, None)
+        bias = None if bs is None else bs[k]
+        if kind is None and bias is None:
+            break
+        st, vals = _act_stage(stages[k], vals, k, kind, kif, bias, a_sz, c_sz)
+        out.append(st)
+        if k + 1 < len(stages):
+            out += [dict(st) for st in stages[k + 1]]
     return RawPipeline.from_stages(out)
+
+
+def _act_stage(layer, vals, k, kind, kif, bias, a_sz, c_sz):
+    """(stage, values handed on) of the bias / activation stage after layer ``k`` (``layer``: its stages) of a chain
+    design: one input op per value, then one constant addition per non-zero bias in value order, then one relu /
+    quantize op per value the activation changes, in value order, reading the value's constant addition when it has one."""
+    last = layer[-1]
+    n = int(last['shape'][1])
+    traced, biased, changed, nxt = _activated_intervals(layer, vals, k, kind, kif, bias)
+    idx = np.asarray(last['out_idxs'], np.int64)
+    of = np.asarray(last['ops_f'], np.float64).reshape(-1, 5)
+    ops_i, ops_f, out_idxs = [], [], np.arange(n, dtype=np.int64)
+    for j in range(n):  # the input ops first, in value order: the traced interval and the solver's latency
+        ops_i.append([j, -1, -1, 0])
+        ops_f.append([*traced[j], float(of[idx[j], 3]) if idx[j] >= 0 else 0.0, 0.0])
+    for j, c in enumerate(biased):  # constant additions: the bias in steps of the result, the tracer's cost
+        if c is not None:
+            out_idxs[j] = len(ops_i)
+            ops_i.append([j, -1, 4, c[4]])
+            ops_f.append([*c[:3], ops_f[j][3], c[3]])
+    for j, a in enumerate(changed):
+        if a is None:
+            continue
+        if a[0] == a[1]:  # (the constant 0)
+            out_idxs[j] = -1
+        else:
+            src = int(out_idxs[j])
+            out_idxs[j] = len(ops_i)
+            ops_i.append([src, -1, 2 if kind == 'relu' else 3, 0])
+            ops_f.append([*a[:3], ops_f[src][3], a[3]])
+    for j, v in enumerate(nxt):
+        if v[0] == v[1] == 0.0:
+            out_idxs[j] = -1
+    st = dict(shape=(n, n), inp_shifts=np.zeros(n, np.int64), out_idxs=out_idxs, out_shifts=np.zeros(n, np.int64), out_negs=np.zeros(n, np.int64),
+              ops_i=np.asarray(ops_i, np.int64).reshape(-1, 4), ops_f=np.asarray(ops_f, np.float32).reshape(-1, 5), adder_size=a_sz, carry_size=c_sz)
+    return st, nxt
 
 
 PRICE_STATUS = ['ok', 'adder slower than the cutoff', 'not supported']  # PipelinePrice.status codes 0, 1, 2

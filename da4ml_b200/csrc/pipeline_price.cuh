@@ -31,8 +31,9 @@ enum PpStatus : int { PP_OK = 0, PP_SLOW_ADDER = 1 /* the tracer's AssertionErro
 // One adder of a design, in dependency-level order.  `node` is its own node id; n0 / n1 the nodes its operands view; q0 /
 // q1 the operand intervals cost_add receives (after FixedVariable.__add__'s sign normalisation, as float32); `flag` 2: an
 // operand is a constant (refused before the latency), 1: the sum is a constant (refused after the latency), 0: neither;
-// 3: not an adder but an activation (relu / quantize, opcodes +-2 / +-3) of node n0 == n1, which keeps its operand's
-// latency (trace/fixed_variable.py:381-384) and whose tracer cost is q0[0].
+// 3: not an adder but an activation (relu / quantize, opcodes +-2 / +-3) or a constant addition (opcode 4) of node n0 ==
+// n1, which keeps its operand's latency (trace/fixed_variable.py:353-359, 381-384) and whose tracer cost is q0[0]; 4: a
+// constant addition of a constant (refused like 2, after the latency).
 struct PpAdd {
     int node, n0, n1, flag;
     float q0[3], q1[3];
@@ -112,10 +113,12 @@ template <bool COST> __device__ __forceinline__ void pp_replay(const PpDesign &d
     for (int l = 0; l < d.n_levels; ++l) {
         for (int k = d.lvl_begin[l] + tid; k < d.lvl_begin[l + 1]; k += nt) {
             const PpAdd a = d.adds[k];
-            if (a.flag == 3) { // an activation (relu / quantize): its operand's latency, no adder
+            if (a.flag >= 3) { // an activation or a constant addition: its operand's latency, no adder
                 t.lat[a.node] = t.lat[a.n0];
                 if (COST)
                     cost_out[a.node] = a.q0[0];
+                if (a.flag == 4) // (of a constant)
+                    atomicMin(&s_fail, ((unsigned long long)a.node << 2) | (unsigned long long)PP_UNSUPPORTED);
                 continue;
             }
             float dl = 0.f, cost = 0.f;
@@ -316,6 +319,22 @@ inline PpAct pp_quantize(double lo, double hi, double step, int k, int i, int f)
     return l == h ? PpAct{1, l, l, st} : PpAct{2, l, h, st};
 }
 
+// _const_f (trace/fixed_variable.py:201-214): the least f in (-32, 32] with c * 2^f an integer; -32 for 0
+inline int pp_const_f(double c) {
+    if (c == 0.0)
+        return -32;
+    int lo = -32, hi = 32;
+    while (hi - lo > 1) {
+        const int mid = (hi + lo) >> 1; // (floor division, as Python's //)
+        const double v = std::ldexp(c, mid);
+        if (v == std::trunc(v))
+            hi = mid;
+        else
+            lo = mid;
+    }
+    return hi;
+}
+
 // sum of minimal_kif (types.py:86-114) of an interval
 inline int pp_kif_bits(double lo, double hi, double step) {
     if (lo == 0.0 && hi == 0.0)
@@ -362,22 +381,25 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
         for (int64_t i = 0; i < S.n_ops; ++i) {
             const int64_t *o = S.ops_i + 4 * i;
             const bool act = o[2] == 2 || o[2] == -2 || o[2] == 3 || o[2] == -3;
+            const bool cadd = o[2] == 4; // a constant addition: data (!= 0, as the tracer records none of 0) steps of its interval
             const bool ok = o[2] == -1 ? (o[0] >= 0 && o[0] < S.n_in && std::abs(S.inp_shifts[o[0]]) <= 512)
                             : (o[2] == 0 || o[2] == 1) ? (o[0] >= 0 && o[0] < i && o[1] >= 0 && o[1] < i && std::abs(o[3]) <= 512)
-                            : act ? (o[0] >= 0 && o[0] < i && o[1] == -1 && o[3] == 0)
-                                  : false;
+                            : act  ? (o[0] >= 0 && o[0] < i && o[1] == -1 && o[3] == 0)
+                            : cadd ? (o[0] >= 0 && o[0] < i && o[1] == -1 && o[3] != 0 && std::llabs(o[3]) < (1ll << 31))
+                                   : false;
             if (!ok)
                 bad("stage " + std::to_string(s) + " op " + std::to_string(i) + ": opcode " + std::to_string(o[2]) + " with operands (" + std::to_string(o[0]) + ", " +
-                    std::to_string(o[1]) + ") is not an adder-graph op (opcodes -1, 0, 1 and the activations +-2, +-3; operands earlier ops, inputs in range)");
-            if (act) { // the op's interval gives the activation's (k, i, f): a finite interval on a power-of-two grid
+                    std::to_string(o[1]) + ") and data " + std::to_string(o[3]) + " is not an adder-graph op (opcodes -1, 0, 1, the activations +-2, +-3 "
+                    "and the constant addition 4 with 0 < |data| < 2^31; operands earlier ops, inputs in range)");
+            if (act || cadd) { // the op's interval gives the activation's (k, i, f): a finite interval on a power-of-two grid
                 const float *q = S.ops_f + 5 * i;
                 const double lo = q[0], hi = q[1], st = q[2];
                 int e = 0;
                 const bool grid = std::isfinite(lo) && std::isfinite(hi) && st > 0 && std::isfinite(st) && std::frexp(st, &e) == 0.5 && lo <= hi &&
                                   std::fabs(lo / st) < 9.0e15 && std::fabs(hi / st) < 9.0e15 && lo / st == std::trunc(lo / st) && hi / st == std::trunc(hi / st);
                 if (!grid)
-                    bad("stage " + std::to_string(s) + " op " + std::to_string(i) + ": the interval of an activation is not a quantized interval (min <= max, "
-                        "multiples of a power-of-two step)");
+                    bad("stage " + std::to_string(s) + " op " + std::to_string(i) + ": the interval of an " + (act ? "activation" : "opcode 4 constant addition") +
+                        " is not a quantized interval (min <= max, multiples of a power-of-two step)");
             }
         }
         for (int64_t k = 0; k < S.n_out; ++k)
@@ -400,6 +422,7 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
     for (int k = 0; k < P.n_in; ++k)
         cur[k] = in_q[3 * k] == in_q[3 * k + 1] ? View{CONST, in_q[3 * k], in_q[3 * k + 1], in_q[3 * k + 2], 1.0} : view_of(k);
     std::vector<int> lvl(P.n_in + 1, 0);
+    std::vector<char> is_cadd(P.n_in + 1, 0); // per node: a constant addition (FixedVariable.opr == 'cadd')
     std::vector<PpAdd> adds;
     for (int64_t s = 0; s < n_stages; ++s) {
         const PpStageIn &S = st[s];
@@ -408,6 +431,40 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
             const int64_t *o = S.ops_i + 4 * i;
             if (o[2] == -1) {
                 buf[i] = scaled(cur[o[0]], std::ldexp(1.0, (int)S.inp_shifts[o[0]]));
+                continue;
+            }
+            if (o[2] == 4) { // FixedVariable._const_add of data * step (CombLogic.__call__, types.py:267-269)
+                const View V = buf[o[0]];
+                const double bias = (double)o[3] * (double)S.ops_f[5 * i + 2];
+                PpAdd a{};
+                a.node = P.n_in + 1 + (int)adds.size();
+                a.n0 = a.n1 = V.node;
+                a.flag = 3;
+                View R{a.node, V.lo + bias, V.hi + bias, std::min(V.step, std::ldexp(1.0, -pp_const_f(bias))), V.f};
+                if (V.lo == V.hi) { // a constant plus a constant: not supported, as an adder of a constant is not
+                    a.flag = 4;
+                    R.step = V.step;
+                } else if (is_cadd[V.node]) {
+                    bad("stage " + std::to_string(s) + " op " + std::to_string(i) + ": an opcode 4 constant addition of a constant addition (the tracer folds "
+                        "the two into one op on the earlier operand; not covered)");
+                }
+                const double d = bias / V.f; // the node's _data, and the tracer's cost ceil(log2(|d| + 2^-f)) + f
+                const int fd = pp_const_f(d);
+                a.q0[0] = (float)(std::ceil(std::log2(std::fabs(d) + std::ldexp(1.0, -fd))) + fd);
+                if (split) {
+                    split->xv.insert(split->xv.end(), {V.lo, V.hi, V.step, V.f});
+                    split->yv.insert(split->yv.end(), {0.0, 0.0, 0.0, 0.0});
+                    split->x.push_back(V.node);
+                    split->y.push_back(-1);
+                    split->opc.push_back(4);
+                    // int(_data / unscaled step): the same through every view of the node
+                    split->data.push_back((int)std::llround(d / (R.step / std::fabs(V.f))));
+                }
+                node_view.push_back(R);
+                lvl.push_back(1 + lvl[V.node]);
+                is_cadd.push_back(1);
+                adds.push_back(a);
+                buf[i] = R;
                 continue;
             }
             if (o[2] != 0 && o[2] != 1) { // relu (+-2) / quantize (+-3) of the operand (negated for the negative opcode)
@@ -451,6 +508,7 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
                 }
                 node_view.push_back(View{a.node, r.lo, r.hi, r.step, std::fabs(V.f)});
                 lvl.push_back(1 + lvl[V.node]);
+                is_cadd.push_back(0);
                 adds.push_back(a);
                 buf[i] = node_view.back();
                 continue;
@@ -489,6 +547,7 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
                 a.flag = 1;
             node_view.push_back(View{a.node, lo, hi, step, f});
             lvl.push_back(1 + std::max(lvl[A.node], lvl[B.node]));
+            is_cadd.push_back(0);
             adds.push_back(a);
             buf[i] = node_view.back();
         }
