@@ -296,9 +296,9 @@ class RawPipeline:
                 cd = dict(zip(COUNTER_NAMES, (int(v) for v in cnt)))
                 cd['phase_cycles'] = [int(v) for v in cnt[16:24]]
                 cd['phase_cycles_max'] = [int(v) for v in cnt[24:32]]
-                ms = np.zeros(63, np.int64)
+                ms = np.zeros(70, np.int64)
                 _check(_L.da4ml_pipeline_stage_milestones(handle, s, _ip(ms)))
-                cd['milestones'] = {250 << k: [int(v) for v in ms[9 * k : 9 * k + 9]] for k in range(7) if ms[9 * k + 8] > 0}
+                cd['milestones'] = {250 << k: [int(v) for v in ms[10 * k : 10 * k + 10]] for k in range(7) if ms[10 * k + 9] > 0}
                 self.counters.append(cd)
             self.device_ms = float(_L.da4ml_pipeline_device_ms(handle))
             self.launches = int(_L.da4ml_pipeline_launches(handle))

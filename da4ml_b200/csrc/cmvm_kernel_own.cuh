@@ -84,8 +84,11 @@ __device__ void solve_problem_own(const ProblemDesc &p, const Ctx &cx, const Own
             b.peak[k] = 0;
             b.nslow[k] = 0;
         }
+        b.phase[8] = 0;
         b.poll_iters = 0;
         ob.pool_used = 0;
+        ob.helped = 0;
+        ob.helped_ovf = 0;
         ob.pass_bits = 0;
         ob.n_ins = 0;
         ob.overflow = 0;
@@ -141,7 +144,8 @@ __device__ void solve_problem_own(const ProblemDesc &p, const Ctx &cx, const Own
     // -- which chunks a substitution invalidates varies wildly from CTA to CTA and step to step, and the group waits for
     // its slowest CTA.  (A CTA of a single warp does both one after the other.)  The last warp (of team R) publishes and
     // collects the exchanges; in a step its lane 0 executes the exchange's release fence while team C still counts:
-    // team C signals barrier 3 once the writes the next step reads (own_update) are done.
+    // team C signals barrier 3 once the writes the next step reads (own_update) are done.  Team R then counts pairs of
+    // the recount's first pass next to team C (barriers 5 and 6, own_recount_help), and the teams join.
     const int rw = nw >= 4 ? nw / 4 : (nw >= 2 ? 1 : 0);
     const bool split = rw > 0;
     const int nt_c = nt - 32 * rw;
@@ -246,7 +250,7 @@ __device__ void solve_problem_own(const ProblemDesc &p, const Ctx &cx, const Own
             DA_LAP(3)
             if (!split && !compacting)
                 refresh_chunks(cx, tm_c, seg0, c0, c1, true, cx.cfg.accounting != 0, thresh);
-            own_recount(p, cx, ox, tm_c, newid, stamp, thresh, best);
+            own_recount(p, cx, ox, tm_c, newid, stamp, thresh, best, split);
             DA_LAP(1)
         }
         else {
@@ -268,6 +272,7 @@ __device__ void solve_problem_own(const ProblemDesc &p, const Ctx &cx, const Own
                     b.phase[2] += clock64() - f0;
                 }
             }
+            own_recount_help(p, cx, ox, pub);
         }
         __syncthreads();
         DA_LAP(4)
@@ -323,10 +328,10 @@ __device__ void solve_problem_own(const ProblemDesc &p, const Ctx &cx, const Own
         DA_LAP(7)
         ++t;
         if (cx.rank == 0 && tid == 0 && t >= 250 && t % 250 == 0 && ((t / 250) & (t / 250 - 1)) == 0 && t / 250 <= 64) {
-            long long *ms = &p.result_meta[META_MILESTONES + 9 * (31 - __clz(t / 250))]; // (diagnostic: where the time of a stage goes)
-            for (int k = 0; k < 8; ++k)
+            long long *ms = &p.result_meta[META_MILESTONES + 10 * (31 - __clz(t / 250))]; // (diagnostic: where the time of a stage goes)
+            for (int k = 0; k < 9; ++k)
                 ms[k] = b.phase[k];
-            ms[8] = clock64() - b.t_start;
+            ms[9] = clock64() - b.t_start;
 #ifdef DA_RECOUNT_PROF
             printf("  recount parts after %d steps (cumulative ms at 1.9 GHz): setup %.2f counting %.2f harvest %.2f\n", t, ob.xphase[0] / 1.9e6, ob.xphase[1] / 1.9e6, ob.xphase[2] / 1.9e6);
 #endif
@@ -347,6 +352,8 @@ __device__ void solve_problem_own(const ProblemDesc &p, const Ctx &cx, const Own
         b.rescanned += (unsigned long long)b.rescan_step;
         atomicAdd((unsigned long long *)&p.result_meta[META_SUM_R], b.r_count);
         atomicAdd((unsigned long long *)&p.result_meta[META_RESCANNED], b.rescanned);
+        atomicAdd((unsigned long long *)&p.result_meta[META_HELPED], (unsigned long long)ob.helped);
+        atomicAdd((unsigned long long *)&p.result_meta[META_HELPED_OVF], (unsigned long long)ob.helped_ovf);
         atomicMax((long long *)&p.result_meta[META_LIST_MAX], (long long)b.list_max);
         for (int k = 0; k < 8; ++k)
             atomicMax((long long *)&p.result_meta[META_PHASEMAX + k], b.phase[k]); // the slowest CTA's total per phase

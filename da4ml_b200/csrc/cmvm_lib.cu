@@ -906,10 +906,10 @@ int da4ml_pipeline_stage_counters(const da4ml_pipeline_t *p, int64_t s, int64_t 
     std::copy(p->impl->stages[s].counters, p->impl->stages[s].counters + 32, counters);
     return DA4ML_OK;
 }
-int da4ml_pipeline_stage_milestones(const da4ml_pipeline_t *p, int64_t s, int64_t out[63]) {
+int da4ml_pipeline_stage_milestones(const da4ml_pipeline_t *p, int64_t s, int64_t out[70]) {
     if (!p || s < 0 || s >= (int64_t)p->impl->stages.size())
         return DA4ML_E_INVALID;
-    std::copy(p->impl->stages[s].counters + META_MILESTONES, p->impl->stages[s].counters + META_MILESTONES + 63, out);
+    std::copy(p->impl->stages[s].counters + META_MILESTONES, p->impl->stages[s].counters + META_MILESTONES + 70, out);
     return DA4ML_OK;
 }
 double da4ml_pipeline_device_ms(const da4ml_pipeline_t *p) { return p ? p->impl->device_ms : 0.0; }

@@ -41,8 +41,10 @@ enum Meta : int {
     META_LIST_MAX = 14,  // longest column list seen
     META_PHASE0 = 16, // 8 words: cycles spent by CTA rank 0 in substitute, recount, refresh, wait1, harvest, publish, wait2, collect
     META_PHASEMAX = 24, // 8 words: the same, maximum over the CTAs of the group
-    META_MILESTONES = 32, // 7 x 9 words: cumulative phase cycles of CTA rank 0 (8 words) + cycles since the problem started, after 250 * 2^k greedy steps (k = 0..6)
-    META_WORDS = 96
+    META_MILESTONES = 32, // 7 x 10 words: cumulative phase cycles of CTA rank 0 (8 words), team R's counting cycles in the first passes of the recount (CTA rank 0), cycles since the problem started; after 250 * 2^k greedy steps (k = 0..6)
+    META_HELPED = 102,     // chunks of 32 recount items team R claimed (all steps, all CTAs)
+    META_HELPED_OVF = 103, // first passes of a recount abandoned after team R had claimed chunks of them
+    META_WORDS = 104
 };
 
 // prep_meta layout (int32 words) written by the prep kernel

@@ -136,7 +136,7 @@ struct BlockCtx {
     unsigned bar_target;
     unsigned epoch;    // exchanges done by this group so far (tags the all-gather slots)
     int scratch_i[4];
-    long long phase[8];
+    long long phase[9]; // the step's phases (DA_LAP), then team R's counting in the recount (own_recount_help)
     long long t_last;
     long long t_start; // start of the greedy loop (thread 0; the milestones of the phase timers)
     long long poll_iters;

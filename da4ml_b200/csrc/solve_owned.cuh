@@ -43,6 +43,10 @@ struct OwnBlock {
     int n_tcol;      // columns touched by the rewritten rows
     int n_ins;       // hash slots claimed in the current pass
     int overflow;    // the current pass ran out of hash slots
+    int claim;       // (column, row) items of the current pass handed out so far (a warp-chunk of 32 per claim)
+    int help_pairs;  // digit pairs team R counted in the step's first pass
+    int help_chunks; // chunks team R claimed there
+    long long helped, helped_ovf; // all steps: chunks team R claimed; first passes abandoned after team R had claimed some
     int pass_bits;   // the owned expressions are counted in 2^pass_bits subsets (adapted from step to step)
     int grew;        // a subset had to be split in this step
     int ins_max;     // most slots claimed by one pass of this step
@@ -592,25 +596,34 @@ __device__ __forceinline__ uint32_t own_pairs_take(const OwnCtx &ox, OwnPairs &s
 }
 
 // Pairs of the rows of one subset of the owned expressions (those with (e / G) mod 2^bits == val) with the rewritten rows,
-// over the touched columns.  The (column, row) items of all touched columns are flattened over the threads of the CTA
-// (tpre = exclusive prefix of the list lengths); the lanes of a warp then draw pairs from their rows in lock step, U at a
-// time.  Returns this thread's digit pairs.
+// over the touched columns.  The (column, row) items of all touched columns are flattened (tpre = exclusive prefix of the
+// list lengths) and handed out a warp-chunk at a time: lane 0 claims the next 32 items of the pass, so that the counting
+// warps -- team C's and, in a step's first pass, team R's once its refresh is done -- finish together however many pairs
+// their rows hold.  The lanes of a warp then draw pairs from their rows in lock step, U at a time.  A pass that is being
+// abandoned hands out nothing more.  Returns this thread's digit pairs; `chunks` counts the warp's claims.
 #ifndef DA_OWN_UNROLL
 #define DA_OWN_UNROLL 2
 #endif
-__device__ int own_count_subset(const ProblemDesc &p, const Ctx &cx, const OwnCtx &ox, const Team &tm, int bits, uint32_t val) {
+__device__ int own_count_subset(const ProblemDesc &p, const Ctx &cx, const OwnCtx &ox, int bits, uint32_t val, int &chunks) {
     DA_DYN_SHARED(da_smem);
-    const int tid = tm.tid, nt = tm.nt, G = cx.cfg.G;
+    const int lane = threadIdx.x & 31, G = cx.cfg.G;
     const uint16_t *tcol = DA_SM(uint16_t, ox.lay.tcol);
     const int *tpre = DA_SM(int, ox.lay.tpre);
-    const OwnBlock &ob = *ox.ob;
+    OwnBlock &ob = *ox.ob;
     const int n_mods = ob.n_mods, n_tcol = ob.n_tcol, nb1 = p.nbits - 1, total = tpre[n_tcol];
     const uint32_t smask = (1u << bits) - 1u;
     const uint32_t m0 = ob.mid[0], m1 = ob.mid[1], m2 = n_mods > 2 ? ob.mid[2] : 0xffffffffu;
     constexpr int U = DA_OWN_UNROLL;
     int pairs = 0;
-    const int total_pad = (total + 31) & ~31; // whole warps enter the loop together
-    for (int item = tid; item < total_pad; item += nt) {
+    while (true) {
+        int base = total;
+        if (lane == 0 && !ld_racy(&ob.overflow))
+            base = smem_add(&ob.claim, 32);
+        base = __shfl_sync(0xffffffffu, base, 0);
+        if (base >= total)
+            break; // (uniform over the warp)
+        ++chunks;
+        const int item = base + lane;
         OwnPairs s;
         s.flags = 0u, s.r = 3, s.ml = s.mh = 0u, s.kbase = 0u, s.o = 0;
         s.P = s.N = s.Pl = s.Nl = s.Ph = s.Nh = 0u;
@@ -695,9 +708,16 @@ __device__ void own_harvest(const ProblemDesc &p, const Ctx &cx, const OwnCtx &o
     }
 }
 
+// Named barriers of the first counting pass when team R helps (every thread of the CTA takes part in both): team C opens
+// the pass with bar.arrive on OWN_BAR_OPEN, and closes it with bar.sync on OWN_BAR_DONE, on which team R arrives.
+#define OWN_BAR_OPEN 5
+#define OWN_BAR_DONE 6
+
 // The whole recount of one step: the owned expressions are processed in subsets small enough for the hash table; a subset
 // that runs out of slots is abandoned (nothing of it has been emitted), the table cleared and the subset split in two.
-__device__ void own_recount(const ProblemDesc &p, const Ctx &cx, const OwnCtx &ox, const Team &tm, uint32_t newid, uint32_t stamp, uint32_t thresh, Best &best) {
+// `helped`: team R joins the first pass (own_recount_help) and team C waits for it before the harvest; team C alone
+// counts every later pass.
+__device__ void own_recount(const ProblemDesc &p, const Ctx &cx, const OwnCtx &ox, const Team &tm, uint32_t newid, uint32_t stamp, uint32_t thresh, Best &best, bool helped) {
     DA_DYN_SHARED(da_smem);
     const int tid = tm.tid, nt = tm.nt, lane = tid & 31;
     OwnBlock &ob = *ox.ob;
@@ -731,6 +751,9 @@ __device__ void own_recount(const ProblemDesc &p, const Ctx &cx, const OwnCtx &o
             ob.sub_stack[ob.sub_top++] = ((uint32_t)b << 16) | (uint32_t)v;
         ob.n_ins = 0;
         ob.overflow = 0;
+        ob.claim = 0;
+        ob.help_pairs = 0;
+        ob.help_chunks = 0;
         ob.grew = 0;
         ob.ins_max = 0;
 #ifdef DA_RECOUNT_PROF
@@ -738,18 +761,26 @@ __device__ void own_recount(const ProblemDesc &p, const Ctx &cx, const OwnCtx &o
 #endif
     }
     team_sync(tm);
+    if (helped)
+        named_arrive(OWN_BAR_OPEN, blockDim.x);
     DA_XLAP(0)
-    int nr = 0;
+    int nr = 0, chunks = 0; // (team C's claims are not reported)
+    bool first = true;
     while (ob.sub_top > 0) { // (uniform: sub_top only changes between the barriers below)
         const uint32_t sv = ob.sub_stack[ob.sub_top - 1];
         const int bits = (int)(sv >> 16);
         const uint32_t val = sv & 0xffffu;
-        const int mine = own_count_subset(p, cx, ox, tm, bits, val);
-        team_sync(tm);
+        const int mine = own_count_subset(p, cx, ox, bits, val, chunks);
+        if (helped && first)
+            team_sync(Team{tid, (int)blockDim.x, OWN_BAR_DONE}); // team R's slots and counts are in the table too
+        else
+            team_sync(tm);
         DA_XLAP(1)
         const bool over = ob.overflow != 0;
         if (!over) {
             nr += mine;
+            if (first && tid == 0)
+                nr += ob.help_pairs;
             own_harvest(p, cx, ox, tm, newid, stamp, thresh, best);
         }
         else {
@@ -773,11 +804,17 @@ __device__ void own_recount(const ProblemDesc &p, const Ctx &cx, const OwnCtx &o
             }
             else
                 ob.ins_max = max(ob.ins_max, ob.n_ins);
+            if (first && ob.help_chunks > 0) {
+                ob.helped += ob.help_chunks;
+                ob.helped_ovf += over ? 1 : 0;
+            }
             ob.n_ins = 0;
             ob.overflow = 0;
+            ob.claim = 0;
         }
         team_sync(tm);
         DA_XLAP(2)
+        first = false;
     }
     if (tid == 0) { // next step's first split: finer after an overflow, coarser when the table stayed almost empty
         if (ob.grew)
@@ -790,6 +827,30 @@ __device__ void own_recount(const ProblemDesc &p, const Ctx &cx, const OwnCtx &o
         nr += __shfl_xor_sync(0xffffffffu, nr, off);
     if (lane == 0 && nr)
         smem_add(&cx.b->r_step, nr);
+}
+
+// Team R's share of the recount, once its refresh (and the exchange's fence) is done: its warps claim items of the step's
+// first pass next to team C until none are left or the pass is being abandoned, then arrive at the pass's end.  They
+// never harvest and never count a later pass; their pairs reach the step's count only if the pass is kept (own_recount).
+// Thread `timer` adds its counting cycles to phase 8.
+__device__ void own_recount_help(const ProblemDesc &p, const Ctx &cx, const OwnCtx &ox, int timer) {
+    OwnBlock &ob = *ox.ob;
+    const int nt = blockDim.x, lane = threadIdx.x & 31;
+    team_sync(Team{0, nt, OWN_BAR_OPEN}); // the prefix of the pass and its state are written
+    const long long t0 = clock64();
+    const uint32_t sv = ob.sub_stack[ob.sub_top - 1];
+    int chunks = 0;
+    int pairs = own_count_subset(p, cx, ox, (int)(sv >> 16), sv & 0xffffu, chunks);
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1)
+        pairs += __shfl_xor_sync(0xffffffffu, pairs, off);
+    if (lane == 0 && chunks > 0) {
+        smem_add(&ob.help_pairs, pairs);
+        smem_add(&ob.help_chunks, chunks);
+    }
+    if ((int)threadIdx.x == timer)
+        cx.b->phase[8] += clock64() - t0;
+    named_arrive(OWN_BAR_DONE, nt);
 }
 
 // ---- D. before the adder trees: the owner lists of all CTAs -> per-column lists in global memory ---------------------

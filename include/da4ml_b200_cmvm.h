@@ -211,10 +211,10 @@ int da4ml_pipeline_stage_copy(
 /* Work counters of one stage, int64[32]: see enum Meta in csrc/cmvm_types.cuh
  * (status, n_ops, T, sum|F_t|, sum R_t, F0, R0, D_final, F_max, compactions, ..., per-phase SM cycles). */
 int da4ml_pipeline_stage_counters(const da4ml_pipeline_t *p, int64_t stage, int64_t counters[32]);
-/* Diagnostic: 7 x 9 words, one group per milestone of 250 * 2^k greedy steps (k = 0..6): cumulative cycles CTA 0 of the
- * problem's group spent in each of the 8 phases of a greedy step, and the cycles since the loop started (zero for
- * milestones the stage did not reach). */
-int da4ml_pipeline_stage_milestones(const da4ml_pipeline_t *p, int64_t stage, int64_t out[63]);
+/* Diagnostic: 7 x 10 words, one group per milestone of 250 * 2^k greedy steps (k = 0..6): cumulative cycles CTA 0 of the
+ * problem's group spent in each of the 8 phases of a greedy step, the cycles its refresh team spent counting digit pairs
+ * of the recount, and the cycles since the loop started (zero for milestones the stage did not reach). */
+int da4ml_pipeline_stage_milestones(const da4ml_pipeline_t *p, int64_t stage, int64_t out[70]);
 /* Device milliseconds spent in this library's kernels for the call that produced p (CUDA events). */
 double da4ml_pipeline_device_ms(const da4ml_pipeline_t *p);
 /* Number of kernel launches issued for the call that produced p. */

@@ -22,10 +22,10 @@ for G in [int(g) for g in os.environ.get('GS', '0,1,2,4').split(',')]:
     print(f'G={G or "auto"}: {nb} x 128x128 int6 wall {dt*1e3:.0f} ms = {nb/dt:.1f} matrices/s | profile {r.profile} | job 0 stage 0: G={c["group_ctas"]} T={T} lcap={c["smem_list_cap"]} '
           f'phases us/step {ph} sum {sum(ph[:2]) + sum(ph[3:6]) + ph[7]:.1f} | stage 1: T={r.counters[1]["T"]} G={r.counters[1]["group_ctas"]}', flush=True)
     ms = c['milestones']
-    prev = [0] * 9
+    prev = [0] * 10
     for k, v in sorted(ms.items()):
         d = [a - b for a, b in zip(v, prev)]
         steps = k - (k // 2 if k > 250 else 0)
-        print(f'    steps ..{k}: {d[8]/1.9e3/steps:.1f} us/step, phases {[round(x/1.9e3/steps,1) for x in d[:8]]}')
+        print(f'    steps ..{k}: {d[9]/1.9e3/steps:.1f} us/step, phases {[round(x/1.9e3/steps,1) for x in d[:8]]}, team R counting {d[8]/1.9e3/steps:.1f}')
         prev = v
 B.set_group_size(0)

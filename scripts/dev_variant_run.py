@@ -31,11 +31,12 @@ mhz = sum(c['phase_cycles'][k] for k in (0, 1, 3, 4, 5, 7)) / (1e3 * raw.device_
 cyc = mhz  # cycles per us
 print(f'{tag}: clock {mhz:.0f} MHz (CTA-0 loop cycles / stage device time), T={T}', flush=True)
 line = f'{tag}: stage G={G} {raw.device_ms:.1f} ms us/step={1e3*raw.device_ms/T:.1f} phases={[round(v/cyc/T,2) for v in c["phase_cycles"]]} max-over-CTAs={[round(v/cyc/T,2) for v in c["phase_cycles_max"]]} dig={digest(raw)}'
-prev = [0] * 9
+prev = [0] * 10
 for k, v in sorted(c['milestones'].items()):
     d = [a - b for a, b in zip(v, prev)]
     steps = k - (k // 2 if k > 250 else 0)
-    print(f'  steps ..{k}: {d[8]/cyc/1e3:.1f} ms, {d[8]/cyc/steps:.1f} us/step, phase us/step={[round(x/cyc/steps,2) for x in d[:8]]}', flush=True)
+    # team R: its warps' share of the recount's first pass, counted once their refresh is done (CTA 0's last warp)
+    print(f'  steps ..{k}: {d[9]/cyc/1e3:.1f} ms, {d[9]/cyc/steps:.1f} us/step, phase us/step={[round(x/cyc/steps,2) for x in d[:8]]} team R counting us/step={d[8]/cyc/steps:.2f}', flush=True)
     prev = v
 B.set_group_size(0)
 if os.environ.get('QUICK'):  # the stage only
