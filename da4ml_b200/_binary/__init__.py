@@ -320,7 +320,13 @@ class RawPipeline:
         r.stages = list(stages)
         return r
 
+    def _no_lookups(self, what: str):
+        if any((np.asarray(st['ops_i']).reshape(-1, 4)[:, 2] == 8).any() for st in self.stages):
+            raise ValueError(f'{what}: this design has opcode 8 lookups, and the Pipeline containers of this package hold no lookup tables '
+                             '(to_binary writes them)')
+
     def to_pipeline(self, types_module=None):
+        self._no_lookups('to_pipeline')
         return pipeline_from_arrays(self.stages, types_module)
 
     # ---- serialisation straight from the flat arrays (SURVEY 8f N3): no per-op Python objects
@@ -340,6 +346,7 @@ class RawPipeline:
 
     def to_json(self) -> str:
         """The text ``Pipeline.save`` writes (reference types.py:678-693)."""
+        self._no_lookups('to_json')
         return stages_to_json(self.stages)
 
     def save(self, path):
@@ -796,13 +803,22 @@ class ChainFront(NetworkFront):
         if activations is None:
             if self.activations is None:
                 raise TypeError('this front was searched without activations: design(p, activations) needs them')
-            activations = self.activations
+            activations = [[_act_tuple(a) for a in seq] for seq in self.activations]
         elif self.activations is not None:
             acts = list(activations)
+            n_outs = [int(r.stages[-1]['shape'][1]) for r in self._raws[p]]
             same = len(acts) == len(self.activations)
-            for k, (act, (kind, kif)) in enumerate(zip(acts, self.activations) if same else ()):
-                a_kind, a_kif = _act_arg(k, act, len(kif))
-                same &= a_kind == kind and np.array_equal(a_kif, kif)
+            for k, (act, mine) in enumerate(zip(acts, self.activations) if same else ()):
+                r = _same_acts(_act_seq(k, act, n_outs[k]), mine)
+                if r is False:  # (kinds, kifs or modes differ: no table comparison can make them the same)
+                    same = False
+                    break
+                if r is None:
+                    same = None
+            if same is None:  # only the 'apply' functions differ: the same tables are the same activations
+                mine = [[_act_tuple(a) for a in seq] for seq in self.activations]
+                a, b = chain_design(self._raws[p], activations, self.biases), chain_design(self._raws[p], mine, self.biases)
+                same = len(a.stages) == len(b.stages) and all(_same_tables(x.get('lookup_tables'), y.get('lookup_tables')) for x, y in zip(a.stages, b.stages))
             if not same:
                 raise ValueError('these activations differ from the ones the front was searched with: its later layers were solved for those')
         return chain_design(self._raws[p], activations, self.biases)
@@ -830,10 +846,10 @@ def _chain_layer(points, state_of, sweeps, state_lats, traced=None, state_qs=Non
     Chains with activations: ``state_qs[s]`` are state ``s``'s qintervals for the reference calls, and ``acted`` is
     ``(group_of, table, ...)`` at every layer but the last (and at the last when it has a bias): ``group_of[p]`` is parent ``p``'s replay group (the parents of one state with the same float64
     input intervals); ``table[g, i]`` is ``None`` when candidate ``i`` under group ``g`` makes a non-zero constant (the
-    pair is dropped), else ``(act_cost, zero, intervals, views)``: the float32 cost of each op of the bias / activation
-    stage in stage order (with a bias: each output's constant addition, then each output's activation op; 0 without
-    one), which outputs become the constant 0, the outputs' intervals after the bias and activation, and their
-    ``[n, 2]`` (factor, cadd) of ``_traced_views``.  A point's cost then continues with ``act_cost`` added in order, and
+    pair is dropped), else ``(act_cost, zero, intervals, views, dls)``: the float32 cost of each op of the bias /
+    activation stage in stage order (with a bias: each output's constant addition, then each activation's op of each
+    output; 0 without one), which outputs become the constant 0, the outputs' intervals after the bias and activations,
+    their ``[n, 2]`` (factor, cadd) of ``_traced_views``, and per output the latency increments of its lookups, in order.  A point's cost then continues with ``act_cost`` added in order, and
     its ``outs`` entry is ``(latencies, intervals, views)``, the latency of a constant 0 being 0."""
     fronts = [np.asarray(sw.front, np.int64) for sw in sweeps]
     if traced is not None:
@@ -874,7 +890,11 @@ def _chain_layer(points, state_of, sweeps, state_lats, traced=None, state_qs=Non
         raws.append([r] if points is None else [*points[4][p], r])
         calls.append([call] if points is None else [*points[5][p], call])
         if acted is not None:
-            _, zero, vals, aux = table[group_of[p], i]
+            _, zero, vals, aux, dls = table[group_of[p], i]
+            o = np.asarray(o).copy()
+            for j, dl in enumerate(dls):  # lookups: the operand's latency plus each increment, in order (no cutoff rule)
+                for d in dl:
+                    o[j] = d + o[j]
             o = (np.where(zero, 0.0, o).astype(o.dtype), vals, aux)
         outs.append(o)
     return cost, lat, choice, outs, raws, calls
@@ -893,7 +913,8 @@ def chain_front(kernels, option_sets, qintervals=None, latencies=None, adder_siz
     layer's outputs.  ``latencies`` are layer 0's input latencies (default zeros).
 
     ``activations[k]`` (``len(kernels) - 1`` of them, in ``chain_design``'s format: ``('relu' | 'quantize', kif[, 'TRN'[,
-    'WRAP']])``) is the op between layer ``k`` and layer ``k + 1``.  With them every layer after the first is solved under
+    'WRAP']])``, ``('apply', fn, kif[, round_mode[, overflow_mode]])``, or a non-empty list of these applied in order) is
+    the op between layer ``k`` and layer ``k + 1``.  With them every layer after the first is solved under
     the intervals a traced model hands it: those of the previous design's traced outputs after the activation (the
     intervals ``chain_design`` gives the activation stage's outputs).  A dead column, or a value that loses all its bits, is
     the tracer's constant 0: the interval (0, 0, 2**32) at latency 0.  Only ``qintervals[0]`` may then be given (``ValueError`` otherwise).
@@ -922,7 +943,9 @@ def chain_front(kernels, option_sets, qintervals=None, latencies=None, adder_siz
     clock.  ``best_stages(n)`` is the cheapest point with at most ``n`` stages.  A point's register bits and register
     stages as one pipeline, with the activations between its layers, are ``price_pipelined(front.design(p,
     activations), c, keep_split=True)`` (``chain_design``).
-    Activations between layers add no latency, as ``relu`` and ``wrap`` in the tracer keep their input's latency.  The
+    ``relu`` and ``quantize`` add no latency, as ``relu`` and ``wrap`` in the tracer keep their input's latency; a lookup
+    (``'apply'``) adds the tracer's ``max(b_in - 6, 1)`` to its operand's latency, with no register-boundary rule, and
+    the next layer's state latencies (and, with a cutoff, the traced ones) include it.  The
     front is the front of the chains explored: the solver is not monotone in its input latencies, so pruning partial
     chains on (cost, latency) is a heuristic and a pruned chain could have led to a better design.  What is reported is
     exact.
@@ -956,7 +979,7 @@ def chain_front(kernels, option_sets, qintervals=None, latencies=None, adder_siz
         acts = list(activations)
         if len(acts) != len(ks) - 1:
             raise ValueError(f'{len(ks)} layers need {len(ks) - 1} activations, got {len(acts)}')
-        acts = [_act_arg(k, act, int(ks[k].shape[1])) for k, act in enumerate(acts)]
+        acts = [_act_seq(k, act, int(ks[k].shape[1])) for k, act in enumerate(acts)]
         for k in range(1, len(ks) if qintervals is not None else 0):
             if qintervals[k] is not None:
                 raise ValueError(f"layer {k}: with activations a layer's qintervals are its traced inputs' (only layer 0's may be given)")
@@ -1006,7 +1029,7 @@ def chain_front(kernels, option_sets, qintervals=None, latencies=None, adder_siz
         bias = None if bs is None else bs[k]
         if acts is not None and (k < len(ks) - 1 or bias is not None):
             t0 = time.perf_counter()
-            acted = _chain_replay(points, state_of, sweeps, traced, k, *(acts[k] if k < len(acts) else (None, None)), bias)
+            acted = _chain_replay(points, state_of, sweeps, traced, k, acts[k] if k < len(acts) else [], bias)
             replayed = dict(replay_ms=(time.perf_counter() - t0) * 1e3, dropped_constant=acted[2]['constant'])
             if bs is not None:
                 replayed.update(dropped_folded=acted[2]['folded'], dropped_inexact=acted[2]['inexact'])
@@ -1033,17 +1056,18 @@ def chain_front(kernels, option_sets, qintervals=None, latencies=None, adder_siz
 _ZERO_QINT = (0.0, 0.0, 2.0**32)  # the tracer's constant 0: FixedVariable gives a constant the step 2**-_const_f(0) = 2**32
 
 
-def _chain_replay(points, state_of, sweeps, traced, k, kind, kif, bias=None):
+def _chain_replay(points, state_of, sweeps, traced, k, seq, bias=None):
     """``_chain_layer``'s ``acted`` for layer ``k`` of a chain with activations: every front candidate (that pricing
-    kept) of every state, replayed through bias ``k`` and activation ``k`` (``kind`` ``None``: the last layer's bias alone)
-    from each distinct float64 input values of the state's parents (at layer 0, the design's own input intervals, as in
-    ``chain_design``).  A table entry is ``None`` for a dropped pair; its reason goes to the returned counts
-    (``constant``, ``folded``, ``inexact``)."""
+    kept) of every state, replayed through bias ``k`` and the activations ``seq`` after layer ``k`` (empty: the last
+    layer's bias alone) from each distinct float64 input values of the state's parents (at layer 0, the design's own
+    input intervals, as in ``chain_design``).  A table entry is ``None`` for a dropped pair; its reason goes to the
+    returned counts (``constant``, ``folded``, ``inexact``)."""
     group_of, groups = [], {}  # parent -> replay group; (state, float64 intervals and views) -> group
     for p, s in enumerate(state_of.tolist()):
         key = None if points is None else np.asarray(points[3][p][1], np.float64).tobytes() + np.asarray(points[3][p][2], np.float64).tobytes()
         group_of.append(groups.setdefault((s, key), len(groups)))
     table, drops = {}, dict(constant=0, folded=0, inexact=0)
+    cache = [{} for _ in seq]  # ('apply' tables by interval and kif, shared by every replay of the layer)
     for (s, key), g in groups.items():
         for i in np.asarray(sweeps[s].front, np.int64).tolist():
             if traced is not None and (s, i) not in traced:
@@ -1056,7 +1080,7 @@ def _chain_replay(points, state_of, sweeps, traced, k, kind, kif, bias=None):
                 n = q.size // 5
                 vals = [(*r[:3], r[3], bool(r[4])) for r in np.concatenate([q[: 3 * n].reshape(n, 3), q[3 * n :].reshape(n, 2)], axis=1).tolist()]
             try:
-                traced_vals, biased, changed, nxt = _activated_intervals(stages, vals, k, kind, kif, bias)
+                traced_vals, biased, changed, nxt = _activated_intervals(stages, vals, k, seq, bias, cache)
             except _FoldedBias:
                 table[g, i] = None
                 drops['folded'] += 1
@@ -1069,13 +1093,14 @@ def _chain_replay(points, state_of, sweeps, traced, k, kind, kif, bias=None):
                 table[g, i] = None
                 drops['constant'] += 1
                 continue
-            act_cost = np.asarray([0.0 if a is None else a[3] for a in changed], np.float32)
-            if bias is not None:  # (stage order: the constant additions, then the activation ops)
-                act_cost = np.concatenate([np.asarray([0.0 if c is None else c[3] for c in biased], np.float32), act_cost])
+            # (stage order: the constant additions, then each activation's ops in value order)
+            act_cost = [np.asarray([0.0 if c is None else c[3] for c in biased], np.float32)] if bias is not None else []
+            act_cost = np.concatenate(act_cost + [np.asarray([0.0 if a is None else a[3] for a in ops], np.float32) for ops in changed]).astype(np.float32)
+            dls = [tuple(int(ops[j][4]) for ops in changed if ops[j] is not None and ops[j][4]) for j in range(len(nxt))]
             zero = np.asarray([v[0] == v[1] for v in nxt], bool)
             vals = [_ZERO_QINT if v[0] == v[1] else v[:3] for v in nxt]
             aux = np.asarray([v[3:] for v in nxt], np.float64).reshape(-1, 2)
-            table[g, i] = (act_cost, zero, np.asarray(vals, np.float64).reshape(-1, 3), aux)
+            table[g, i] = (act_cost, zero, np.asarray(vals, np.float64).reshape(-1, 3), aux, dls)
     return group_of, table, drops
 
 
@@ -1229,20 +1254,22 @@ def _input_intervals(stages) -> list:
     return vals
 
 
-def _activated_intervals(stages, vals, k: int, kind, kif, bias=None):
+def _activated_intervals(stages, vals, k: int, seq, bias=None, cache=None):
     """One step of the tracer's interval replay of a chain: layer ``k``'s design (``stages``) on inputs ``vals``
     (``_traced_views``), then bias ``k`` (``None`` or ``[n_out]`` float64, added to every output with
-    ``FixedVariable._const_add``), then activation ``k`` (``kind``, ``[n_out, 3]`` kif; ``kind`` ``None``: none, as after
+    ``FixedVariable._const_add``), then the activations of ``seq`` (``_act_seq`` specs, in order; empty: none, as after
     the last layer) on every output.  Returns ``(traced, biased, acts, nxt)``: ``traced[j]`` is output ``j``'s (lo, hi,
     step); ``biased[j]`` is ``None`` without a bias op, else the (lo, hi, step, cost, data) of the constant addition the
-    tracer records (``_bias_op``); ``acts[j]`` is ``None`` when the activation leaves the (biased) value unchanged, else
-    the (lo, hi, step, cost) of the op the tracer records for it (cost ``sum(kif) / 2`` for relu, 0 for quantize), or (0.0,
-    0.0, 1.0, 0.0) for the constant 0 (a dead column, or a format with no bits left); ``nxt[j]`` is the value handed on,
-    as (lo, hi, step, factor, cadd).  ``_ConstantValue`` when a value is or becomes any other constant, ``_FoldedBias``
-    for a bias the tracer folds.  The one Python copy of these rules (the C++ copy is ``pp_prepare``'s)."""
+    tracer records (``_bias_op``); ``acts[a][j]`` is ``None`` when activation ``a`` of the sequence leaves value ``j``
+    unchanged, else the (lo, hi, step, cost, dl, table) of the op the tracer records for it (relu: cost ``sum(kif) / 2``,
+    quantize: 0, both dl 0 and table ``None``; apply: the lookup's cost, latency increment and table, ``_apply_op``), or
+    (0.0, 0.0, 1.0, 0.0, 0, None) for the constant 0 (a dead column, or a format with no bits left); ``nxt[j]`` is the
+    value handed on, as (lo, hi, step, factor, cadd).  ``_ConstantValue`` when a value is or becomes any other constant,
+    ``_FoldedBias`` for a bias the tracer folds.  ``cache``: the tables of ``'apply'`` activations by (interval, kif), one
+    dict per activation of ``seq``.  The one Python copy of these rules (the C++ copy is ``pp_prepare``'s)."""
     views = _traced_views(stages, vals)
     traced = [v[:3] for v in views]
-    biased, acts, nxt = [], [], []
+    biased, cur = [], []
     for j, v in enumerate(views):
         b = 0.0 if bias is None else float(bias[j])
         if b != 0.0:
@@ -1251,26 +1278,49 @@ def _activated_intervals(stages, vals, k: int, kind, kif, bias=None):
             v = (*r[:3], v[3], True)
         else:
             biased.append(None)
-        lo, hi, st = v[:3]
-        if lo == hi:
-            if lo != 0.0 or hi != 0.0:
-                raise _ConstantValue(f'activation {k}: output {j} of layer {k} is the constant {lo} (only the constant 0 is covered)')
-            acts.append(None if kind is None else (0.0, 0.0, 1.0, 0.0))
-            nxt.append((0.0, 0.0, 1.0, 1.0, False))
-            continue
-        r = None if kind is None else _activate(kind, lo, hi, st, *(int(x) for x in kif[j]))
-        if r is None:
-            acts.append(None)
-            nxt.append(v)
-        elif r[0] == r[1]:
-            if r[0] != 0.0:
-                raise _ConstantValue(f'activation {k}: output {j} becomes the constant {r[0]} (only the constant 0 is covered)')
-            acts.append((0.0, 0.0, 1.0, 0.0))
-            nxt.append((0.0, 0.0, 1.0, 1.0, False))
-        else:
-            acts.append((*r, sum(_kif_prop(*r)) / 2 if kind == 'relu' else 0.0))
-            nxt.append((*r, abs(v[3]), False))
-    return traced, biased, acts, nxt
+        cur.append(v)
+    cache = [{} for _ in seq] if cache is None else cache
+    acts = []
+    for a, spec in enumerate(seq):
+        kind, kif = spec[:2]
+        ops, nxt = [], []
+        for j, v in enumerate(cur):
+            lo, hi, st = v[:3]
+            if kind == 'apply':
+                r = _apply_op(j, k, v, kif[j], *spec[2:], cache[a])
+                if r is None:
+                    ops.append((0.0, 0.0, 1.0, 0.0, 0, None))
+                    nxt.append((0.0, 0.0, 1.0, 1.0, False))
+                else:
+                    ops.append(r)
+                    nxt.append((*r[:3], 1.0, False))
+                continue
+            if lo == hi:
+                if lo != 0.0 or hi != 0.0:
+                    raise _ConstantValue(f'activation {k}: output {j} of layer {k} is the constant {lo} (only the constant 0 is covered)')
+                ops.append((0.0, 0.0, 1.0, 0.0, 0, None))
+                nxt.append((0.0, 0.0, 1.0, 1.0, False))
+                continue
+            r = _activate(kind, lo, hi, st, *(int(x) for x in kif[j]))
+            if r is None:
+                ops.append(None)
+                nxt.append(v)
+            elif r[0] == r[1]:
+                if r[0] != 0.0:
+                    raise _ConstantValue(f'activation {k}: output {j} becomes the constant {r[0]} (only the constant 0 is covered)')
+                ops.append((0.0, 0.0, 1.0, 0.0, 0, None))
+                nxt.append((0.0, 0.0, 1.0, 1.0, False))
+            else:
+                ops.append((*r, sum(_kif_prop(*r)) / 2 if kind == 'relu' else 0.0, 0, None))
+                nxt.append((*r, abs(v[3]), False))
+        acts.append(ops)
+        cur = nxt
+    for j, v in enumerate(cur):
+        if not seq and v[0] == v[1]:
+            if v[0] != 0.0 or v[1] != 0.0:
+                raise _ConstantValue(f'activation {k}: output {j} of layer {k} is the constant {v[0]} (only the constant 0 is covered)')
+            cur[j] = (0.0, 0.0, 1.0, 1.0, False)
+    return traced, biased, acts, cur
 
 
 def _bias_arg(k: int, b, n: int):
@@ -1302,17 +1352,33 @@ def _biases_arg(biases, n_outs):
     return bs if any(b is not None for b in bs) else None
 
 
+_APPLY_ROUND = ('TRN', 'RND')
+_APPLY_OVERFLOW = ('WRAP', 'SAT', 'SAT_SYM')
+
+
 def _act_arg(k: int, act, n: int):
-    """(kind, [n, 3] int64 kif) of activation ``k`` of ``chain_design``."""
-    if not isinstance(act, (tuple, list)) or len(act) not in (2, 3, 4):
-        raise ValueError(f"activation {k}: expected ('quantize' | 'relu', kif[, round_mode[, overflow_mode]]), got {act!r}")
-    kind, kif, *modes = act
-    if kind not in ('quantize', 'relu'):
-        raise ValueError(f"activation {k}: {kind!r} is not 'quantize' or 'relu'")
-    if len(modes) > 0 and str(modes[0]).upper() != 'TRN':
-        raise ValueError(f'activation {k}: rounding mode {modes[0]!r} is not covered (only TRN)')
-    if len(modes) > 1 and str(modes[1]).upper() != 'WRAP':
-        raise ValueError(f'activation {k}: overflow mode {modes[1]!r} is not covered (only WRAP)')
+    """(kind, [n, 3] int64 kif) of activation ``k`` of ``chain_design``; for ``'apply'``, (kind, kif, fn, round_mode,
+    overflow_mode)."""
+    if not isinstance(act, (tuple, list)) or len(act) not in ((3, 4, 5) if len(act) and isinstance(act[0], str) and act[0] == 'apply' else (2, 3, 4)):
+        raise ValueError(f"activation {k}: expected ('quantize' | 'relu', kif[, round_mode[, overflow_mode]]) or ('apply', fn, kif[, round_mode[, overflow_mode]]), got {act!r}")
+    if isinstance(act[0], str) and act[0] == 'apply':
+        kind, fn, kif, *modes = act
+        if not callable(fn):
+            raise ValueError(f"activation {k}: the function of 'apply' must be callable, got {fn!r}")
+        rnd = str(modes[0]).upper() if len(modes) > 0 else 'TRN'
+        ovf = str(modes[1]).upper() if len(modes) > 1 else 'WRAP'
+        if rnd not in _APPLY_ROUND:
+            raise ValueError(f"activation {k}: rounding mode {modes[0]!r} of 'apply' is not one of {', '.join(_APPLY_ROUND)}")
+        if ovf not in _APPLY_OVERFLOW:
+            raise ValueError(f"activation {k}: overflow mode {modes[1]!r} of 'apply' is not one of {', '.join(_APPLY_OVERFLOW)}")
+    else:
+        kind, kif, *modes = act
+        if kind not in ('quantize', 'relu'):
+            raise ValueError(f"activation {k}: {kind!r} is not 'quantize', 'relu' or 'apply'")
+        if len(modes) > 0 and str(modes[0]).upper() != 'TRN':
+            raise ValueError(f'activation {k}: rounding mode {modes[0]!r} is not covered (only TRN)')
+        if len(modes) > 1 and str(modes[1]).upper() != 'WRAP':
+            raise ValueError(f'activation {k}: overflow mode {modes[1]!r} is not covered (only WRAP)')
     a = np.asarray(kif)
     if a.dtype == bool:
         a = a.astype(np.int64)
@@ -1327,7 +1393,110 @@ def _act_arg(k: int, act, n: int):
         raise ValueError(f"activation {k}: k must be 0 or 1" + (" (0 for 'relu': its output is unsigned)" if kind == 'relu' else ''))
     if (np.abs(a[:, 1:]) > 64).any():
         raise ValueError(f'activation {k}: i and f must be within [-64, 64]')
-    return kind, a
+    return (kind, a) if kind != 'apply' else (kind, a, fn, rnd, ovf)
+
+
+def _act_tuple(spec) -> tuple:
+    """The ``chain_design`` activation tuple of an ``_act_arg`` spec."""
+    return ('apply', spec[2], spec[1], *spec[3:]) if spec[0] == 'apply' else tuple(spec)
+
+
+def _act_seq(k: int, act, n: int) -> list:
+    """Activation ``k`` of ``chain_design`` / ``chain_front`` as a list of ``_act_arg`` specs, applied in order: one
+    activation tuple (its first element a ``str``) or a non-empty list of them."""
+    if isinstance(act, (tuple, list)) and len(act) and isinstance(act[0], str):
+        return [_act_arg(k, act, n)]
+    if not isinstance(act, (tuple, list)) or len(act) == 0:
+        raise ValueError(f'activation {k}: expected an activation tuple or a non-empty list of them, got {act!r}')
+    return [_act_arg(k, a, n) for a in act]
+
+
+def _same_acts(a: list, b: list) -> bool | None:
+    """Whether two ``_act_seq`` lists are the same activations: ``False`` when kinds, kifs or modes differ, ``True`` when
+    they are equal and every ``'apply'`` function is the same object, ``None`` when only the functions differ (the caller
+    compares the tables they give)."""
+    if len(a) != len(b) or any(x[0] != y[0] or not np.array_equal(x[1], y[1]) or x[3:] != y[3:] for x, y in zip(a, b)):
+        return False
+    return None if any(x[0] == 'apply' and x[2] is not y[2] for x, y in zip(a, b)) else True
+
+
+def fixed_quantize(x, k, i, f, overflow_mode: str = 'WRAP', round_mode: str = 'TRN') -> np.ndarray:
+    """The numeric fixed-point quantizer the tracer applies to an ``apply`` table (``_quantize``): round to the step
+    ``2**-f`` (TRN: floor, RND: floor of ``x + step / 2``), then bring the result into ``[-k * 2**i, 2**i - 2**-f]``
+    (WRAP: modulo ``2**(k + i)``; SAT: clip; SAT_SYM: clip to ``[-k * (2**i - 2**-f), 2**i - 2**-f]``).  A format with
+    ``k + i + f <= 0`` gives 0."""
+    x = np.asarray(x, np.float64)
+    if k + i + f <= 0:
+        return np.zeros_like(x)
+    st = 2.0**-f
+    y = np.floor(x / st + (0.5 if round_mode == 'RND' else 0.0)) * st
+    hi = 2.0**i - st
+    if overflow_mode == 'WRAP':
+        lo = -k * 2.0**i
+        return np.mod(y - lo, 2.0 ** (i + k)) + lo
+    lo = -k * 2.0**i if overflow_mode == 'SAT' else -k * hi
+    return np.clip(y, lo, hi)
+
+
+def _interpret_as(x, k: int, i: int, f: int):
+    """``interpret_as`` of the tracer (trace/fixed_variable.py:100-110): integers read as two's complement (k, i, f)."""
+    b = k + i + f
+    bias = 2.0 ** (b - 1) * k
+    return 2.0**-f * (np.floor(x + bias) % 2.0**b - bias)
+
+
+def _lsb_locs(x: np.ndarray) -> np.ndarray:
+    """``get_lsb_loc`` of every element (its float32 value): the exponent of its lowest set bit, 127 for 0."""
+    b = np.asarray(x, np.float32).view(np.uint32).astype(np.int64)
+    e, m = (b >> 23) & 0xFF, (b & 0x7FFFFF) + (1 << 23)
+    tz = np.log2(m & -m).astype(np.int64)
+    return np.where(np.asarray(x, np.float32) == 0, 127, e + tz - 150)
+
+
+def _make_table(values: np.ndarray):
+    """``to_spec`` of the tracer (trace/fixed_variable.py:72-79): (sha256 hex, int32 table, out_qint)."""
+    import hashlib
+
+    f_out = int(-_lsb_locs(values).min())
+    ints = (values * 2.0**f_out).astype(np.int32)
+    h = hashlib.sha256(ints.data)
+    h.update(f'{f_out}'.encode())
+    return h.hexdigest(), ints, (float(np.min(values)), float(np.max(values)), float(2.0**-f_out))
+
+
+def _apply_op(j: int, k: int, v, kif, fn, rnd: str, ovf: str, cache: dict):
+    """What the tracer's ``x.apply(fn).quantize(k, i, f, ovf, rnd)`` makes of value ``v`` = (lo, hi, step, factor, cadd):
+    the table over the value's interval (reversed for a negative factor), each entry quantized (``fixed_quantize``), its
+    ``to_spec``, then ``FixedVariable.lookup``.  Returns ``None`` for the constant 0, else (lo, hi, step, cost, dl, table)
+    with the tracer's lookup cost and latency increment (trace/fixed_variable.py:331-340) and ``table`` = (sha, int32
+    values, out_qint).  ``_ConstantValue`` for a non-zero constant.  ``cache`` holds the tables of one activation by
+    (interval, kif), as the tracer's ``local_tables``."""
+    from math import ceil
+
+    lo, hi, st, fac = v[:4]
+    a, b = (lo, hi) if fac >= 0 else (hi, lo)
+    kk, ii, ff = (int(x) for x in kif)
+    key = (a, b, st if lo != hi else 0.0, kk, ii, ff)
+    if key not in cache:
+        n = round(abs(b - a) / st) + 1 if lo != hi else 1
+        x = np.linspace(a, b, n)
+        y = np.asarray(fn(x), np.float64)
+        if y.shape != x.shape:
+            raise ValueError(f'activation {k}: the function of \'apply\' gave shape {y.shape} for an input of shape {x.shape}')
+        if not np.isfinite(y).all():
+            raise ValueError(f"activation {k}: the function of 'apply' gave a value that is not finite on the interval [{min(a, b)}, {max(a, b)}]")
+        cache[key] = _make_table(fixed_quantize(y, kk, ii, ff, ovf, rnd))
+    table = cache[key]
+    o_lo, o_hi, o_st = table[2]
+    if o_lo == o_hi:
+        if o_lo != 0.0:
+            raise _ConstantValue(f'activation {k}: output {j} becomes the constant {o_lo} (only the constant 0 is covered)')
+        return None
+    b_in, b_out = sum(_kif_prop(lo, hi, st)), sum(_kif_prop(o_lo, o_hi, o_st))
+    cost = 2 ** max(b_in - 5, 0) * ceil(b_out / 2)
+    if b_in < 5:
+        cost *= b_in / 5
+    return o_lo, o_hi, o_st, float(cost), max(b_in - 6, 1), table
 
 
 def chain_design(designs, activations, biases=None) -> RawPipeline:
@@ -1343,6 +1512,18 @@ def chain_design(designs, activations, biases=None) -> RawPipeline:
     ``quantize(k, i, f)``, with ``kif`` one ``(k, i, f)`` triple for every output or an ``[n_out_k, 3]`` int array (``k``
     is 0 for relu).  Rounding is TRN and overflow WRAP; an optional third and fourth element may name them, and any other
     mode is a ``ValueError``.
+
+    ``('apply', fn, kif[, round_mode[, overflow_mode]])`` is what the tracer makes of ``x.apply(fn).quantize(k, i, f,
+    overflow_mode, round_mode)``: per value a lookup table (opcode 8) of ``fn`` over the value's traced interval (in
+    reversed order when the tracer's view of the value has a negative factor), each entry quantized to ``(k, i, f)``
+    (``fixed_quantize``: TRN / RND, WRAP / SAT / SAT_SYM, which change only the table values).  ``fn`` maps a float64
+    array to an array of the same shape.  Values with equal tables share one; a stage with lookups has
+    ``lookup_tables`` (per table its int32 values and ``out_qint``, numbered by first use), and a lookup op's ``data`` is
+    its table's index.  A lookup costs ``2**max(b_in - 5, 0) * ceil(b_out / 2)`` (times ``b_in / 5`` when ``b_in < 5``)
+    and adds ``max(b_in - 6, 1)`` to its operand's latency.  A value whose table has one value becomes that constant:
+    0 is a dead column, any other is refused.  ``activations[k]`` may be a non-empty list of activations, applied in
+    order, e.g. ``[('quantize', (1, 2, 3)), ('apply', np.tanh, (1, 0, 6))]`` (a pre-quantizer keeps the table small); a
+    one-element list is the activation itself.
 
     An activation stage has one input op per value (opcode -1, the value's interval ``Pipeline.out_qint`` and latency), and
     one op per value the activation changes, with the fields the tracer records for it: opcode 2 (relu) or 3 (quantize)
@@ -1380,29 +1561,37 @@ def chain_design(designs, activations, biases=None) -> RawPipeline:
         if stages[k - 1][-1]['shape'][1] != stages[k][0]['shape'][0]:
             raise ValueError(f"layer {k - 1} has {stages[k - 1][-1]['shape'][1]} outputs but layer {k} has {stages[k][0]['shape'][0]} inputs")
     n_outs = [int(st[-1]['shape'][1]) for st in stages]
-    kinds = [_act_arg(k, act, n_outs[k]) for k, act in enumerate(acts)]
+    kinds = [_act_seq(k, act, n_outs[k]) for k, act in enumerate(acts)]
     bs = _biases_arg(biases, n_outs)
     vals = _input_intervals(stages[0])
     out = [dict(st) for st in stages[0]]
     for k in range(len(stages)):
-        kind, kif = kinds[k] if k < len(kinds) else (None, None)
+        seq = kinds[k] if k < len(kinds) else []
         bias = None if bs is None else bs[k]
-        if kind is None and bias is None:
+        if not seq and bias is None:
             break
-        st, vals = _act_stage(stages[k], vals, k, kind, kif, bias, a_sz, c_sz)
+        st, vals = _act_stage(stages[k], vals, k, seq, bias, a_sz, c_sz)
         out.append(st)
         if k + 1 < len(stages):
             out += [dict(st) for st in stages[k + 1]]
     return RawPipeline.from_stages(out)
 
 
-def _act_stage(layer, vals, k, kind, kif, bias, a_sz, c_sz):
+def _same_tables(a, b) -> bool:
+    """Whether two stages' ``lookup_tables`` (or ``None``) hold the same tables in the same order."""
+    a, b = a or [], b or []
+    return len(a) == len(b) and all(np.array_equal(x['table'], y['table']) and tuple(x['out_qint']) == tuple(y['out_qint']) for x, y in zip(a, b))
+
+
+def _act_stage(layer, vals, k, seq, bias, a_sz, c_sz):
     """(stage, values handed on) of the bias / activation stage after layer ``k`` (``layer``: its stages) of a chain
-    design: one input op per value, then one constant addition per non-zero bias in value order, then one relu /
-    quantize op per value the activation changes, in value order, reading the value's constant addition when it has one."""
+    design: one input op per value, then one constant addition per non-zero bias in value order, then for each
+    activation of ``seq`` in order one op per value it changes, in value order, reading the value's latest op.  A
+    lookup's ``data`` is its table's index in the stage's ``lookup_tables`` (tables numbered by first use, one per
+    distinct content)."""
     last = layer[-1]
     n = int(last['shape'][1])
-    traced, biased, changed, nxt = _activated_intervals(layer, vals, k, kind, kif, bias)
+    traced, biased, changed, nxt = _activated_intervals(layer, vals, k, seq, bias)
     idx = np.asarray(last['out_idxs'], np.int64)
     of = np.asarray(last['ops_f'], np.float64).reshape(-1, 5)
     ops_i, ops_f, out_idxs = [], [], np.arange(n, dtype=np.int64)
@@ -1414,21 +1603,33 @@ def _act_stage(layer, vals, k, kind, kif, bias, a_sz, c_sz):
             out_idxs[j] = len(ops_i)
             ops_i.append([j, -1, 4, c[4]])
             ops_f.append([*c[:3], ops_f[j][3], c[3]])
-    for j, a in enumerate(changed):
-        if a is None:
-            continue
-        if a[0] == a[1]:  # (the constant 0)
-            out_idxs[j] = -1
-        else:
+    tables, index = [], {}
+    for (kind, *_), ops in zip(seq, changed):
+        for j, a in enumerate(ops):
+            if a is None:
+                continue
+            if a[0] == a[1]:  # (the constant 0)
+                out_idxs[j] = -1
+                continue
             src = int(out_idxs[j])
             out_idxs[j] = len(ops_i)
-            ops_i.append([src, -1, 2 if kind == 'relu' else 3, 0])
-            ops_f.append([*a[:3], ops_f[src][3], a[3]])
+            if kind == 'apply':
+                sha, ints, out_q = a[5]
+                if sha not in index:
+                    index[sha] = len(tables)
+                    tables.append(dict(table=ints, out_qint=out_q))
+                ops_i.append([src, -1, 8, index[sha]])
+                ops_f.append([*a[:3], a[4] + float(np.float32(ops_f[src][3])), a[3]])
+            else:
+                ops_i.append([src, -1, 2 if kind == 'relu' else 3, 0])
+                ops_f.append([*a[:3], ops_f[src][3], a[3]])
     for j, v in enumerate(nxt):
         if v[0] == v[1] == 0.0:
             out_idxs[j] = -1
     st = dict(shape=(n, n), inp_shifts=np.zeros(n, np.int64), out_idxs=out_idxs, out_shifts=np.zeros(n, np.int64), out_negs=np.zeros(n, np.int64),
               ops_i=np.asarray(ops_i, np.int64).reshape(-1, 4), ops_f=np.asarray(ops_f, np.float32).reshape(-1, 5), adder_size=a_sz, carry_size=c_sz)
+    if tables:
+        st['lookup_tables'] = tables
     return st, nxt
 
 
@@ -1503,15 +1704,55 @@ class PipelinePrice:
                              self.cutoffs, out_lat, self.profile, splits)  # fmt: skip
 
 
-def _split_stages(meta, outs, shifts, negs, ops_i, ops_f, adder_size, carry_size) -> list[dict]:
-    """Stage dicts (fresh arrays) of one split from its concatenated tables."""
+def _split_stages(meta, outs, shifts, negs, ops_i, ops_f, adder_size, carry_size, tables=None) -> list[dict]:
+    """Stage dicts (fresh arrays) of one split from its concatenated tables.  ``tables``: the design's lookup tables
+    (``_design_tables``), which the split's opcode 8 ops index; each stage then gets the ones it uses as its own
+    ``lookup_tables``, in the order of their first use in the split (the order of the traced model's tables that
+    ``remap_table_idxs`` of ``to_pipeline`` keeps), and its ops are renumbered to match."""
+    from math import ceil
+
     stages, o, r = [], 0, 0
+    first = {}  # design table -> first use in the split's op order, which is the order of the traced model's ops
+    for d in ops_i[ops_i[:, 2] == 8, 3].tolist() if tables else ():
+        first.setdefault(d, len(first))
     for n_in, n_out, n_ops in meta.tolist():
-        stages.append(dict(shape=(n_in, n_out), inp_shifts=np.zeros(n_in, np.int64), out_idxs=outs[o : o + n_out].copy(), out_shifts=shifts[o : o + n_out].copy(),
-                           out_negs=negs[o : o + n_out].astype(bool), ops_i=ops_i[r : r + n_ops].copy(), ops_f=ops_f[r : r + n_ops].copy(), adder_size=adder_size,
-                           carry_size=carry_size))  # fmt: skip
+        st = dict(shape=(n_in, n_out), inp_shifts=np.zeros(n_in, np.int64), out_idxs=outs[o : o + n_out].copy(), out_shifts=shifts[o : o + n_out].copy(),
+                  out_negs=negs[o : o + n_out].astype(bool), ops_i=ops_i[r : r + n_ops].copy(), ops_f=ops_f[r : r + n_ops].copy(), adder_size=adder_size,
+                  carry_size=carry_size)  # fmt: skip
+        lut = st['ops_i'][:, 2] == 8
+        for q in np.flatnonzero(lut).tolist():  # a lookup's cost is a double (m * b_in / 5 for b_in < 5); the kernels hold a float
+            m = ceil(sum(_kif_prop(*st['ops_f'][q, :3].tolist())) / 2)
+            st['ops_f'][q, 4] = next((m * (b / 5) for b in range(1, 5) if np.float32(m * (b / 5)) == np.float32(st['ops_f'][q, 4])), st['ops_f'][q, 4])
+        if tables and lut.any():
+            used = sorted(set(st['ops_i'][lut, 3].tolist()), key=first.get)
+            remap = {g: i for i, g in enumerate(used)}
+            st['ops_i'][lut, 3] = [remap[g] for g in st['ops_i'][lut, 3].tolist()]
+            st['lookup_tables'] = [dict(table=tables[g]['table'].copy(), out_qint=tuple(tables[g]['out_qint'])) for g in used]
+        stages.append(st)
         o, r = o + n_out, r + n_ops
     return stages
+
+
+def _design_tables(stages):
+    """(tables, per-stage index maps) of a design: its distinct lookup tables over all stages, numbered by first use in
+    op order, and for every stage the map from its own table indices to these."""
+    tables, index, maps = [], {}, []
+    for st in stages:
+        own = st.get('lookup_tables') or []
+        m = {}
+        oi = np.asarray(st['ops_i'], np.int64).reshape(-1, 4)
+        for d in oi[oi[:, 2] == 8, 3].tolist():
+            if not 0 <= d < len(own):
+                raise ValueError(f'an opcode 8 lookup reads table {d}, but its stage has {len(own)} lookup tables')
+            if d not in m:
+                t = own[d]
+                key = (np.asarray(t['table'], np.int32).tobytes(), tuple(float(v) for v in t['out_qint']))
+                if key not in index:
+                    index[key] = len(tables)
+                    tables.append(dict(table=np.asarray(t['table'], np.int32), out_qint=key[1]))
+                m[d] = index[key]
+        maps.append(m)
+    return tables, maps
 
 
 def _take_splits(designs, m, info, copy) -> list:
@@ -1531,7 +1772,8 @@ def _take_splits(designs, m, info, copy) -> list:
             outs, shifts, negs = np.zeros(n_outs, np.int64), np.zeros(n_outs, np.int64), np.zeros(n_outs, np.int64)
             ops_i, ops_f = np.zeros((n_rows, 4), np.int64), np.zeros((n_rows, 5), np.float64)
             copy(d * m + j, meta, outs, shifts, negs, ops_i, ops_f)
-            row.append((0, (meta, outs, shifts, negs, ops_i, ops_f, int(stages[0]['adder_size']), int(stages[0]['carry_size']))))
+            tables = _design_tables(stages)[0] if any('lookup_tables' in st for st in stages) else None
+            row.append((0, (meta, outs, shifts, negs, ops_i, ops_f, int(stages[0]['adder_size']), int(stages[0]['carry_size']), tables)))
         out.append(row)
     return out
 
@@ -1553,6 +1795,15 @@ def _price_args(designs, latency_cutoff, latencies) -> dict:
     if cut.size == 0:
         raise ValueError('price_pipelined needs at least one latency cutoff')
     stages = [st for d in designs for st in d]
+    if any('lookup_tables' in st or (np.asarray(st['ops_i']).reshape(-1, 4)[:, 2] == 8).any() for st in stages):
+        stages = []  # (lookups read the design's tables, numbered over all its stages: _design_tables)
+        for d in designs:
+            for st, m in zip(d, _design_tables(d)[1]):
+                if m:
+                    st = dict(st, ops_i=np.asarray(st['ops_i'], np.int64).reshape(-1, 4).copy())
+                    lut = st['ops_i'][:, 2] == 8
+                    st['ops_i'][lut, 3] = [m[v] for v in st['ops_i'][lut, 3].tolist()]
+                stages.append(st)
     meta = np.asarray([[st['shape'][0], st['shape'][1], len(st['ops_i']), st['carry_size'], st['adder_size']] for st in stages], np.int64).reshape(-1, 5)
     cat = lambda key, w: np.ascontiguousarray(np.concatenate([np.asarray(st[key], np.int64).reshape(-1, w) for st in stages]).ravel())  # noqa: E731
     ops_f = np.ascontiguousarray(np.concatenate([np.asarray(st['ops_f'], np.float32).reshape(-1, 5) for st in stages]).ravel())

@@ -33,7 +33,9 @@ enum PpStatus : int { PP_OK = 0, PP_SLOW_ADDER = 1 /* the tracer's AssertionErro
 // operand is a constant (refused before the latency), 1: the sum is a constant (refused after the latency), 0: neither;
 // 3: not an adder but an activation (relu / quantize, opcodes +-2 / +-3) or a constant addition (opcode 4) of node n0 ==
 // n1, which keeps its operand's latency (trace/fixed_variable.py:353-359, 381-384) and whose tracer cost is q0[0]; 4: a
-// constant addition of a constant (refused like 2, after the latency).
+// constant addition of a constant (refused like 2, after the latency); 5: a lookup (opcode 8) of node n0 == n1, whose
+// latency is its operand's plus q0[1] (max(b_in - 6, 1), no register-boundary rule: trace/fixed_variable.py:331-340) and
+// whose tracer cost is q0[0].
 struct PpAdd {
     int node, n0, n1, flag;
     float q0[3], q1[3];
@@ -113,8 +115,8 @@ template <bool COST> __device__ __forceinline__ void pp_replay(const PpDesign &d
     for (int l = 0; l < d.n_levels; ++l) {
         for (int k = d.lvl_begin[l] + tid; k < d.lvl_begin[l + 1]; k += nt) {
             const PpAdd a = d.adds[k];
-            if (a.flag >= 3) { // an activation or a constant addition: its operand's latency, no adder
-                t.lat[a.node] = t.lat[a.n0];
+            if (a.flag >= 3) { // an activation, a constant addition or a lookup: no adder
+                t.lat[a.node] = a.flag == 5 ? pp_add((double)a.q0[1], t.lat[a.n0]) : t.lat[a.n0];
                 if (COST)
                     cost_out[a.node] = a.q0[0];
                 if (a.flag == 4) // (of a constant)
@@ -382,23 +384,28 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
             const int64_t *o = S.ops_i + 4 * i;
             const bool act = o[2] == 2 || o[2] == -2 || o[2] == 3 || o[2] == -3;
             const bool cadd = o[2] == 4; // a constant addition: data (!= 0, as the tracer records none of 0) steps of its interval
+            // a lookup: data the index of its table.  The tables themselves do not reach the kernels (a lookup's cost and
+            // latency depend on intervals only), so the caller checks the index against them: the Python host does
+            // (_design_tables), and a direct C ABI caller must.
+            const bool lut = o[2] == 8;
             const bool ok = o[2] == -1 ? (o[0] >= 0 && o[0] < S.n_in && std::abs(S.inp_shifts[o[0]]) <= 512)
                             : (o[2] == 0 || o[2] == 1) ? (o[0] >= 0 && o[0] < i && o[1] >= 0 && o[1] < i && std::abs(o[3]) <= 512)
                             : act  ? (o[0] >= 0 && o[0] < i && o[1] == -1 && o[3] == 0)
                             : cadd ? (o[0] >= 0 && o[0] < i && o[1] == -1 && o[3] != 0 && std::llabs(o[3]) < (1ll << 31))
+                            : lut  ? (o[0] >= 0 && o[0] < i && o[1] == -1 && o[3] >= 0 && o[3] < (1ll << 31))
                                    : false;
             if (!ok)
                 bad("stage " + std::to_string(s) + " op " + std::to_string(i) + ": opcode " + std::to_string(o[2]) + " with operands (" + std::to_string(o[0]) + ", " +
                     std::to_string(o[1]) + ") and data " + std::to_string(o[3]) + " is not an adder-graph op (opcodes -1, 0, 1, the activations +-2, +-3 "
-                    "and the constant addition 4 with 0 < |data| < 2^31; operands earlier ops, inputs in range)");
-            if (act || cadd) { // the op's interval gives the activation's (k, i, f): a finite interval on a power-of-two grid
+                    "and the constant addition 4 with 0 < |data| < 2^31, the lookup 8 with a table index; operands earlier ops, inputs in range)");
+            if (act || cadd || lut) { // the op's interval gives the activation's (k, i, f): a finite interval on a power-of-two grid
                 const float *q = S.ops_f + 5 * i;
                 const double lo = q[0], hi = q[1], st = q[2];
                 int e = 0;
                 const bool grid = std::isfinite(lo) && std::isfinite(hi) && st > 0 && std::isfinite(st) && std::frexp(st, &e) == 0.5 && lo <= hi &&
                                   std::fabs(lo / st) < 9.0e15 && std::fabs(hi / st) < 9.0e15 && lo / st == std::trunc(lo / st) && hi / st == std::trunc(hi / st);
                 if (!grid)
-                    bad("stage " + std::to_string(s) + " op " + std::to_string(i) + ": the interval of an " + (act ? "activation" : "opcode 4 constant addition") +
+                    bad("stage " + std::to_string(s) + " op " + std::to_string(i) + ": the interval of an " + (act ? "activation" : cadd ? "opcode 4 constant addition" : "opcode 8 lookup") +
                         " is not a quantized interval (min <= max, multiples of a power-of-two step)");
             }
         }
@@ -465,6 +472,37 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
                 is_cadd.push_back(1);
                 adds.push_back(a);
                 buf[i] = R;
+                continue;
+            }
+            if (o[2] == 8) { // FixedVariable.lookup of the operand (CombLogic.__call__): the table's interval, factor 1
+                const View V = buf[o[0]];
+                if (V.lo == V.hi)
+                    bad("stage " + std::to_string(s) + " op " + std::to_string(i) + ": an opcode 8 lookup of a constant (the tracer makes a constant of it; not covered)");
+                const float *q = S.ops_f + 5 * i;
+                PpAdd a{};
+                a.node = P.n_in + 1 + (int)adds.size();
+                a.n0 = a.n1 = V.node;
+                a.flag = 5;
+                // get_cost_and_latency: b_in the kif bits of the operand as the tracer sees it, b_out the result's
+                const int b_in = pp_kif_prop_bits(V.lo, V.hi, V.step), b_out = pp_kif_prop_bits(q[0], q[1], q[2]);
+                double cost = std::ldexp(1.0, std::max(b_in - 5, 0)) * std::ceil(b_out / 2.0);
+                if (b_in < 5)
+                    cost *= b_in / 5.0;
+                a.q0[0] = (float)cost;
+                a.q0[1] = (float)std::max(b_in - 6, 1);
+                if (split) {
+                    split->xv.insert(split->xv.end(), {V.lo, V.hi, V.step, V.f});
+                    split->yv.insert(split->yv.end(), {0.0, 0.0, 0.0, 0.0});
+                    split->x.push_back(V.node);
+                    split->y.push_back(-1);
+                    split->opc.push_back(8);
+                    split->data.push_back((int)o[3]);
+                }
+                node_view.push_back(View{a.node, (double)q[0], (double)q[1], (double)q[2], 1.0});
+                lvl.push_back(1 + lvl[V.node]);
+                is_cadd.push_back(0);
+                adds.push_back(a);
+                buf[i] = node_view.back();
                 continue;
             }
             if (o[2] != 0 && o[2] != 1) { // relu (+-2) / quantize (+-3) of the operand (negated for the negative opcode)

@@ -284,14 +284,23 @@ def stage_to_binary(st, version: int = 0) -> np.ndarray:
     oi = np.asarray(st['ops_i'], dtype=np.int64).reshape(-1, 4)
     of = np.asarray(st['ops_f'], dtype=np.float32).reshape(-1, 5)
     n_ops = oi.shape[0]
-    header = np.concatenate([[1, version, n_in, n_out, n_ops, 0], np.asarray(st['inp_shifts'], dtype=np.int64), np.asarray(st['out_idxs'], dtype=np.int64), np.asarray(st['out_shifts'], dtype=np.int64), (np.asarray(st['out_negs']) != 0).astype(np.int64)]).astype(np.int32)
+    tables = st.get('lookup_tables') or []
+    header = np.concatenate([[1, version, n_in, n_out, n_ops, len(tables)], np.asarray(st['inp_shifts'], dtype=np.int64), np.asarray(st['out_idxs'], dtype=np.int64), np.asarray(st['out_shifts'], dtype=np.int64), (np.asarray(st['out_negs']) != 0).astype(np.int64)]).astype(np.int32)
     code = np.zeros((n_ops, 8), dtype=np.int32)
     if n_ops:
         code[:, 0] = oi[:, 2]
         code[:, 1:3] = oi[:, 0:2]
         code[:, 3:5] = np.ascontiguousarray(oi[:, 3]).view(np.int32).reshape(-1, 2)
         code[:, 5:8] = minimal_kif_array(of[:, 0:3].astype(np.float64))
-    return np.concatenate([header, code.ravel()])
+        for r in np.flatnonzero(oi[:, 2] == 8).tolist():  # lookup: pad_left << 32 | table index (LookupTable._get_pads)
+            lo, _, step = of[oi[r, 0], 0:3].astype(np.float64)
+            k, i, _ = code[oi[r, 0], 5:8].tolist()
+            pad = round((lo + 2.0**i) / step) if k else round(lo / step)
+            code[r, 3:5] = np.asarray([(pad << 32) | int(oi[r, 3])], np.int64).view(np.int32)
+    if not tables:
+        return np.concatenate([header, code.ravel()])
+    ints = [np.asarray(t['table'], np.int32) for t in tables]
+    return np.concatenate([header, code.ravel(), np.asarray([len(t) for t in ints], np.int32), *ints]).astype(np.int32)
 
 
 def stage_to_jsonable(st) -> list:

@@ -241,7 +241,11 @@ int da4ml_pipeline_profile(const da4ml_pipeline_t *p, double out[8]);
  * latencies (0.0 for a dead column).  Not ok: stages = reg_bits = -1, latencies NaN.  profile (NULL to skip) =
  * {device_ms, launches}.  A design may also hold the relu / quantize ops of a chain design (opcodes +-2 / +-3: id0 an
  * earlier op, id1 -1, data 0, the op's interval on a power-of-two grid giving its (k, i, f); TRN / WRAP), replayed as
- * CombLogic.__call__ replays them.  Arguments are checked on the host before any device call: shapes, other opcodes,
+ * CombLogic.__call__ replays them, constant additions (opcode 4) and lookups (opcode 8: id0 an earlier op, id1 -1, data
+ * its table's index in [0, 2^31), the op's interval the table's out_qint on a power-of-two grid).  The tables do not
+ * cross this ABI: a lookup's cost and latency depend on intervals only, and the caller must check each lookup's index
+ * against its own tables (the split hands the index back unchanged).  Arguments are checked on the host before any
+ * device call: shapes, other opcodes,
  * operands, bad activation intervals, an activation of a non-zero constant and cutoffs <= 0 give DA4ML_E_INVALID. */
 int da4ml_pipeline_price(
     int64_t n_designs, const int64_t *n_stages, const int64_t *stage_meta, const int64_t *inp_shifts,
