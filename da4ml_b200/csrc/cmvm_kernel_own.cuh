@@ -429,9 +429,17 @@ __device__ __forceinline__ void solve_own_kernel_body(const ProblemDesc *probs, 
         bctx.epoch = 0u;
     }
     __syncthreads();
+    // The problem's descriptor is read all through a greedy step, and every acquire of the exchange or of the group
+    // barrier invalidates L1: from global memory each field would be an L2 round trip again (an op-record lookup chases
+    // two of them before its own load).  So the CTA works from a copy in shared memory.
+    DA_SHARED_VAR(ProblemDesc, pds);
     const int group = blockIdx.x / cfg.G, n_groups = gridDim.x / cfg.G;
-    for (int pi = group; pi < n_probs; pi += n_groups)
-        solve_problem_own(probs[pi], cxs, oxs);
+    for (int pi = group; pi < n_probs; pi += n_groups) {
+        if (threadIdx.x == 0)
+            pds = probs[pi]; // (the previous problem ended with a group barrier: nobody reads the old copy any more)
+        __syncthreads();
+        solve_problem_own(pds, cxs, oxs);
+    }
 }
 __global__ void __launch_bounds__(512, 1) cmvm_solve_kernel(const ProblemDesc *probs, int n_probs, const GroupWs *wss, const OwnWs *ows, LaunchCfg cfg, int n_out_max, int e_cap_max, int lcap, int hlog, int narrow) {
     solve_own_kernel_body(probs, n_probs, wss, ows, cfg, n_out_max, e_cap_max, lcap, hlog, narrow);
