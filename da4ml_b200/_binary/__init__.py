@@ -833,7 +833,7 @@ class ChainFront(NetworkFront):
         return copy.deepcopy(self._calls[p])
 
 
-def _chain_layer(points, state_of, sweeps, state_lats, traced=None, state_qs=None, acted=None):
+def _chain_layer(points, state_of, sweeps, state_lats, traced=None, state_qs=None, acted=None, cutoff=0.0):
     """Extend the points of the layers so far by the next layer and prune.  ``points`` is ``None`` at layer 0, else
     ``(cost, lat, choice, outs, raws, calls)``; ``state_of[p]`` is the index of point ``p``'s input-latency state in
     ``sweeps`` and ``state_lats`` (lists of Python floats); at layer 0 there is one state and ``state_of == [0]``.
@@ -849,7 +849,8 @@ def _chain_layer(points, state_of, sweeps, state_lats, traced=None, state_qs=Non
     pair is dropped), else ``(act_cost, zero, intervals, views, dls)``: the float32 cost of each op of the bias /
     activation stage in stage order (with a bias: each output's constant addition, then each activation's op of each
     output; 0 without one), which outputs become the constant 0, the outputs' intervals after the bias and activations,
-    their ``[n, 2]`` (factor, cadd) of ``_traced_views``, and per output the latency increments of its lookups, in order.  A point's cost then continues with ``act_cost`` added in order, and
+    their ``[n, 2]`` (factor, cadd) of ``_traced_views``, and per output its latency steps in order (a lookup's increment, or a leaky
+    ReLU's (condition dlat, mux dlat), applied at ``cutoff`` by ``_act_latency``).  A point's cost then continues with ``act_cost`` added in order, and
     its ``outs`` entry is ``(latencies, intervals, views)``, the latency of a constant 0 being 0."""
     fronts = [np.asarray(sw.front, np.int64) for sw in sweeps]
     if traced is not None:
@@ -892,9 +893,9 @@ def _chain_layer(points, state_of, sweeps, state_lats, traced=None, state_qs=Non
         if acted is not None:
             _, zero, vals, aux, dls = table[group_of[p], i]
             o = np.asarray(o).copy()
-            for j, dl in enumerate(dls):  # lookups: the operand's latency plus each increment, in order (no cutoff rule)
+            for j, dl in enumerate(dls):  # lookups and leaky ReLUs, in order (_act_latency)
                 for d in dl:
-                    o[j] = d + o[j]
+                    o[j] = _act_latency(float(o[j]), d, cutoff) if isinstance(d, tuple) else d + o[j]
             o = (np.where(zero, 0.0, o).astype(o.dtype), vals, aux)
         outs.append(o)
     return cost, lat, choice, outs, raws, calls
@@ -913,7 +914,8 @@ def chain_front(kernels, option_sets, qintervals=None, latencies=None, adder_siz
     layer's outputs.  ``latencies`` are layer 0's input latencies (default zeros).
 
     ``activations[k]`` (``len(kernels) - 1`` of them, in ``chain_design``'s format: ``('relu' | 'quantize', kif[, 'TRN'[,
-    'WRAP']])``, ``('apply', fn, kif[, round_mode[, overflow_mode]])``, or a non-empty list of these applied in order) is
+    'WRAP']])``, ``('apply', fn, kif[, round_mode[, overflow_mode]])``, ``('leaky_relu', alpha)``, or a non-empty list of
+    these applied in order) is
     the op between layer ``k`` and layer ``k + 1``.  With them every layer after the first is solved under
     the intervals a traced model hands it: those of the previous design's traced outputs after the activation (the
     intervals ``chain_design`` gives the activation stage's outputs).  A dead column, or a value that loses all its bits, is
@@ -1035,7 +1037,7 @@ def chain_front(kernels, option_sets, qintervals=None, latencies=None, adder_siz
                 replayed.update(dropped_folded=acted[2]['folded'], dropped_inexact=acted[2]['inexact'])
         elif acts is not None:
             replayed = dict(replay_ms=0.0, dropped_constant=0, **({} if bs is None else dict(dropped_folded=0, dropped_inexact=0)))
-        points = _chain_layer(points, state_of, sweeps, lats, traced, None if acts is None else state_qs, acted)
+        points = _chain_layer(points, state_of, sweeps, lats, traced, None if acts is None else state_qs, acted, c)
         if len(points[0]) == 0:
             if replayed.get('dropped_constant') or replayed.get('dropped_folded') or replayed.get('dropped_inexact'):
                 raise ValueError(f'layer {k}: every front candidate is slower than the latency cutoff {c}, makes an output of bias / activation {k} a '
@@ -1095,13 +1097,37 @@ def _chain_replay(points, state_of, sweeps, traced, k, seq, bias=None):
                 continue
             # (stage order: the constant additions, then each activation's ops in value order)
             act_cost = [np.asarray([0.0 if c is None else c[3] for c in biased], np.float32)] if bias is not None else []
-            act_cost = np.concatenate(act_cost + [np.asarray([0.0 if a is None else a[3] for a in ops], np.float32) for ops in changed]).astype(np.float32)
-            dls = [tuple(int(ops[j][4]) for ops in changed if ops[j] is not None and ops[j][4]) for j in range(len(nxt))]
+            act_cost = np.concatenate(act_cost + [np.asarray(_op_costs(ops), np.float32) for ops in changed]).astype(np.float32)
+            dls = [tuple((a.cond[4], a.mux[4]) if isinstance(a, _Mux) else int(a[4]) for a in (ops[j] for ops in changed)
+                         if a is not None and not isinstance(a, _View) and (isinstance(a, _Mux) or a[4])) for j in range(len(nxt))]
             zero = np.asarray([v[0] == v[1] for v in nxt], bool)
             vals = [_ZERO_QINT if v[0] == v[1] else v[:3] for v in nxt]
             aux = np.asarray([v[3:] for v in nxt], np.float64).reshape(-1, 2)
             table[g, i] = (act_cost, zero, np.asarray(vals, np.float64).reshape(-1, 3), aux, dls)
     return group_of, table, drops
+
+
+def _op_costs(ops) -> list:
+    """The cost of every op one activation records, in stage order: per value (0 for none); for a leaky ReLU every
+    condition adder, then every mux."""
+    if any(isinstance(a, (_Mux, _View)) for a in ops):
+        return [a.cond[3] if isinstance(a, _Mux) else 0.0 for a in ops] + [a.mux[3] if isinstance(a, _Mux) else 0.0 for a in ops]
+    return [0.0 if a is None else a[3] for a in ops]
+
+
+def _act_latency(lat: float, dl, c: float) -> float:
+    """An output's latency after one latency step of ``_chain_replay``'s ``dls``: a lookup's increment (no cutoff rule), or
+    a leaky ReLU's (condition dlat, mux dlat): the condition adder under the tracer's register-boundary rule at cutoff
+    ``c`` (trace/fixed_variable.py:373-379), then the mux, ``max`` of its operands plus its dlat, with no rule."""
+    from math import ceil
+
+    if not isinstance(dl, tuple):
+        return dl + lat
+    d, m = float(dl[0]), float(dl[1])
+    cond = d + lat
+    if c > 0 and ceil(cond / c) > ceil(lat / c):
+        cond = ceil(lat / c) * c + d
+    return max(lat, cond) + m
 
 
 def _kif_prop(lo: float, hi: float, step: float) -> tuple[int, int, int]:
@@ -1262,7 +1288,8 @@ def _activated_intervals(stages, vals, k: int, seq, bias=None, cache=None):
     step); ``biased[j]`` is ``None`` without a bias op, else the (lo, hi, step, cost, data) of the constant addition the
     tracer records (``_bias_op``); ``acts[a][j]`` is ``None`` when activation ``a`` of the sequence leaves value ``j``
     unchanged, else the (lo, hi, step, cost, dl, table) of the op the tracer records for it (relu: cost ``sum(kif) / 2``,
-    quantize: 0, both dl 0 and table ``None``; apply: the lookup's cost, latency increment and table, ``_apply_op``), or
+    quantize: 0, both dl 0 and table ``None``; apply: the lookup's cost, latency increment and table, ``_apply_op``;
+    leaky_relu: a ``_Mux`` or a ``_View``, ``_leaky_op``), or
     (0.0, 0.0, 1.0, 0.0, 0, None) for the constant 0 (a dead column, or a format with no bits left); ``nxt[j]`` is the
     value handed on, as (lo, hi, step, factor, cadd).  ``_ConstantValue`` when a value is or becomes any other constant,
     ``_FoldedBias`` for a bias the tracer folds.  ``cache``: the tables of ``'apply'`` activations by (interval, kif), one
@@ -1286,6 +1313,11 @@ def _activated_intervals(stages, vals, k: int, seq, bias=None, cache=None):
         ops, nxt = [], []
         for j, v in enumerate(cur):
             lo, hi, st = v[:3]
+            if kind == 'leaky_relu':
+                r, w = _leaky_op(j, k, v, kif, int(stages[0]['adder_size']), int(stages[0]['carry_size']))
+                ops.append(r)
+                nxt.append(w)
+                continue
             if kind == 'apply':
                 r = _apply_op(j, k, v, kif[j], *spec[2:], cache[a])
                 if r is None:
@@ -1358,7 +1390,17 @@ _APPLY_OVERFLOW = ('WRAP', 'SAT', 'SAT_SYM')
 
 def _act_arg(k: int, act, n: int):
     """(kind, [n, 3] int64 kif) of activation ``k`` of ``chain_design``; for ``'apply'``, (kind, kif, fn, round_mode,
-    overflow_mode)."""
+    overflow_mode); for ``'leaky_relu'``, (kind, alpha)."""
+    if isinstance(act, (tuple, list)) and len(act) and isinstance(act[0], str) and act[0] == 'leaky_relu':
+        a = act[1] if len(act) == 2 else None
+        ok = isinstance(a, (int, float, np.integer, np.floating)) and not isinstance(a, (bool, np.bool_))
+        if ok:
+            a = float(a)
+            ok = bool(np.isfinite(a)) and 0.0 < a < 1.0 and np.frexp(a)[0] == 0.5
+        if not ok:
+            raise ValueError(f"activation {k}: ('leaky_relu', alpha) needs alpha a power of two with 0 < alpha < 1 (the tracer multiplies by any "
+                             f'other with adders), got {act!r}')
+        return ('leaky_relu', a)
     if not isinstance(act, (tuple, list)) or len(act) not in ((3, 4, 5) if len(act) and isinstance(act[0], str) and act[0] == 'apply' else (2, 3, 4)):
         raise ValueError(f"activation {k}: expected ('quantize' | 'relu', kif[, round_mode[, overflow_mode]]) or ('apply', fn, kif[, round_mode[, overflow_mode]]), got {act!r}")
     if isinstance(act[0], str) and act[0] == 'apply':
@@ -1374,7 +1416,7 @@ def _act_arg(k: int, act, n: int):
     else:
         kind, kif, *modes = act
         if kind not in ('quantize', 'relu'):
-            raise ValueError(f"activation {k}: {kind!r} is not 'quantize', 'relu' or 'apply'")
+            raise ValueError(f"activation {k}: {kind!r} is not 'quantize', 'relu', 'apply' or 'leaky_relu'")
         if len(modes) > 0 and str(modes[0]).upper() != 'TRN':
             raise ValueError(f'activation {k}: rounding mode {modes[0]!r} is not covered (only TRN)')
         if len(modes) > 1 and str(modes[1]).upper() != 'WRAP':
@@ -1499,6 +1541,57 @@ def _apply_op(j: int, k: int, v, kif, fn, rnd: str, ovf: str, cache: dict):
     return o_lo, o_hi, o_st, float(cost), max(b_in - 6, 1), table
 
 
+class _Mux(tuple):
+    """The two ops the tracer's ``np.maximum(x, alpha * x)`` records for one value: ``cond`` = (lo, hi, step, cost, dlat) of
+    the condition adder ``x - alpha * x`` and ``mux`` = (lo, hi, step, cost, dlat) of the MSB mux of ``alpha * x`` and ``x``
+    on it (the intervals those of the values the tracer hands on), ``qint`` the interval ``max_of`` hands ``msb_mux``."""
+
+    cond = property(lambda self: self[0])
+    mux = property(lambda self: self[1])
+    qint = property(lambda self: self[2])
+
+
+class _View(tuple):
+    """A leaky ReLU the tracer answers with the view ``alpha * x`` (no op): ``shift`` = log2(alpha)."""
+
+    shift = property(lambda self: self[0])
+
+
+def _leaky_op(j: int, k: int, v, alpha: float, a_sz: int, c_sz: int):
+    """What the tracer's ``np.maximum(x, alpha * x)`` (``FixedVariable.max_of``, trace/fixed_variable.py:902-920, then
+    ``msb_mux`` with ``zt_sensitive=False``, :788-859) makes of value ``v`` = (lo, hi, step, factor, cadd), ``alpha`` a
+    power of two in (0, 1): (op, value handed on).  ``op`` is ``None`` when it is ``x`` itself (``lo >= alpha * hi``), a
+    ``_View`` when it is the view ``alpha * x`` (``hi <= alpha * lo``), the constant-0 record for 0, else a ``_Mux``.
+    ``_ConstantValue`` for a non-zero constant."""
+    from math import floor, log2
+
+    lo, hi, st, fac, cadd = v
+    if lo == hi:
+        if lo != 0.0:
+            raise _ConstantValue(f'activation {k}: output {j} of layer {k} is the constant {lo} (only the constant 0 is covered)')
+        return (0.0, 0.0, 1.0, 0.0, 0, None), (0.0, 0.0, 1.0, 1.0, False)
+    ax = (alpha * lo, alpha * hi, alpha * st, alpha * fac)  # (_pow2_mul: a view of the same node)
+    if lo >= ax[1]:
+        return None, v
+    if hi <= ax[0]:
+        return _View((int(log2(alpha)),)), (*ax, cadd)
+    x = (lo, hi, st, fac)
+    nax = (0.0 - ax[1], 0.0 - ax[0], ax[2], -ax[3])
+    X, Y = (x, nax) if fac > 0 else (nax, x)  # (FixedVariable.__add__: the operand with a positive factor leads)
+    c_dl, c_cost = cost_add(X[:3], Y[:3], 0, False, a_sz, c_sz)
+    cond = (X[0] + Y[0], X[1] + Y[1], min(st, ax[2]), c_cost, c_dl)
+    qint = (max(lo, ax[0]), max(hi, ax[1]), min(st, ax[2]))
+    A, B, q, neg = ax, x, qint, ax[3] < 0
+    if neg:  # (msb_mux of -a, -b under the mirrored qint, seen negated)
+        A, B, q = (0.0 - A[1], 0.0 - A[0], A[2], -A[3]), (0.0 - B[1], 0.0 - B[0], B[2], -B[3]), (0.0 - qint[1], 0.0 - qint[0], qint[2])
+    step = min(A[2], B[2])
+    m_lo = max(floor(q[0] / step) * step, min(A[0], B[0]))
+    m_hi = min(floor(q[1] / step) * step, max(A[1], B[1]))
+    m_dl, m_cost = cost_add(A[:3], B[:3], 0, False, a_sz, c_sz)
+    mux = (0.0 - m_hi, 0.0 - m_lo, step, m_cost / 2, m_dl) if neg else (m_lo, m_hi, step, m_cost / 2, m_dl)
+    return _Mux((cond, mux, qint)), (*mux[:3], ax[3], False)
+
+
 def chain_design(designs, activations, biases=None) -> RawPipeline:
     """A chain of solver designs with a relu or quantizer between consecutive layers, as ONE design: layer 0's stages, an
     activation stage, layer 1's stages, and so on.  ``price_pipelined`` prices and splits it as the reference's tracer
@@ -1524,6 +1617,12 @@ def chain_design(designs, activations, biases=None) -> RawPipeline:
     0 is a dead column, any other is refused.  ``activations[k]`` may be a non-empty list of activations, applied in
     order, e.g. ``[('quantize', (1, 2, 3)), ('apply', np.tanh, (1, 0, 6))]`` (a pre-quantizer keeps the table small); a
     one-element list is the activation itself.
+
+    ``('leaky_relu', alpha)``, ``alpha`` a power of two in (0, 1), is what the tracer makes of ``np.maximum(x, alpha *
+    x)``: per value a condition adder (opcode 1, ``x - alpha * x``) and an MSB mux (opcode 6) of ``alpha * x`` and ``x``
+    on it, with the tracer's intervals, costs and latencies, or no op where the tracer returns ``x`` or the view ``alpha *
+    x`` (``_leaky_op``).  A leaky ReLU ends its stage: the condition adders close it, and the next stage starts with the
+    muxes (DESIGN.md, "Leaky ReLU in whole chains").
 
     An activation stage has one input op per value (opcode -1, the value's interval ``Pipeline.out_qint`` and latency), and
     one op per value the activation changes, with the fields the tracer records for it: opcode 2 (relu) or 3 (quantize)
@@ -1571,7 +1670,7 @@ def chain_design(designs, activations, biases=None) -> RawPipeline:
         if not seq and bias is None:
             break
         st, vals = _act_stage(stages[k], vals, k, seq, bias, a_sz, c_sz)
-        out.append(st)
+        out += st
         if k + 1 < len(stages):
             out += [dict(st) for st in stages[k + 1]]
     return RawPipeline.from_stages(out)
@@ -1584,11 +1683,15 @@ def _same_tables(a, b) -> bool:
 
 
 def _act_stage(layer, vals, k, seq, bias, a_sz, c_sz):
-    """(stage, values handed on) of the bias / activation stage after layer ``k`` (``layer``: its stages) of a chain
+    """(stages, values handed on) of the bias / activation stage after layer ``k`` (``layer``: its stages) of a chain
     design: one input op per value, then one constant addition per non-zero bias in value order, then for each
     activation of ``seq`` in order one op per value it changes, in value order, reading the value's latest op.  A
     lookup's ``data`` is its table's index in the stage's ``lookup_tables`` (tables numbered by first use, one per
-    distinct content)."""
+    distinct content).  A leaky ReLU adds its condition adders (opcode 1, ``x - alpha * x``) in value order and ends the
+    stage; the stage outputs every value (a ``_View`` at ``out_shift = log2(alpha)``), then for each mux ``alpha * x``
+    (``out_shift = log2(alpha)``) and its condition, and the next stage starts with one input op per output and the muxes
+    in value order (opcode 6 of ``alpha * x`` and ``x`` with shift 0 on the condition): a DAIS mux shifts only its second
+    operand, so ``alpha * x`` has to reach it as a value of its own."""
     last = layer[-1]
     n = int(last['shape'][1])
     traced, biased, changed, nxt = _activated_intervals(layer, vals, k, seq, bias)
@@ -1603,8 +1706,51 @@ def _act_stage(layer, vals, k, seq, bias, a_sz, c_sz):
             out_idxs[j] = len(ops_i)
             ops_i.append([j, -1, 4, c[4]])
             ops_f.append([*c[:3], ops_f[j][3], c[3]])
-    tables, index = [], {}
-    for (kind, *_), ops in zip(seq, changed):
+    stages, tables, index = [], [], {}
+    n_in = n
+
+    def close(extra=(), shifts=None):
+        st = dict(shape=(n_in, n + len(extra)), inp_shifts=np.zeros(n_in, np.int64), out_idxs=np.concatenate([out_idxs, np.asarray(extra, np.int64)]),
+                  out_shifts=np.zeros(n + len(extra), np.int64) if shifts is None else np.asarray(shifts, np.int64), out_negs=np.zeros(n + len(extra), np.int64),
+                  ops_i=np.asarray(ops_i, np.int64).reshape(-1, 4), ops_f=np.asarray(ops_f, np.float32).reshape(-1, 5), adder_size=a_sz, carry_size=c_sz)  # fmt: skip
+        if tables:
+            st['lookup_tables'] = list(tables)
+        stages.append(st)
+
+    for (kind, *rest), ops in zip(seq, changed):
+        if kind == 'leaky_relu':
+            muxes, conds = [j for j, a in enumerate(ops) if isinstance(a, _Mux)], {}
+            for j in muxes:  # the condition adders: x - 2**log2(alpha) * x, the tracer's cost
+                src = int(out_idxs[j])
+                conds[j] = len(ops_i)
+                ops_i.append([src, src, 1, int(np.log2(rest[0]))])
+                ops_f.append([*ops[j].cond[:3], ops_f[src][3] + ops[j].cond[4], ops[j].cond[3]])
+            sh = int(np.log2(rest[0]))
+            extra = [v for j in muxes for v in (int(out_idxs[j]), conds[j])]
+            shifts = [sh if isinstance(a, _View) else 0 for a in ops] + [v for _ in muxes for v in (sh, 0)]
+            q_out = []  # (interval, latency) of every output of the closing stage, as the next stage's input ops record them
+            for o, sft in zip(list(out_idxs) + extra, shifts):
+                if o < 0:
+                    q_out.append((0.0, 0.0, 1.0, 0.0))
+                    continue
+                lo, hi, st_ = (float(np.float32(x)) * 2.0**sft for x in ops_f[o][:3])
+                q_out.append((lo, hi, st_, float(np.float32(ops_f[o][3]))))
+            close(extra, shifts)
+            n_in, tables, index = len(q_out), [], {}
+            ops_i = [[j, -1, -1, 0] for j in range(n_in)]
+            ops_f = [[*q[:3], q[3], 0.0] for q in q_out]
+            out_idxs = np.arange(n, dtype=np.int64)
+            for t, j in enumerate(muxes):  # the muxes: alpha * x (input n + 2t), x (input j), the condition (input n + 2t + 1)
+                m = ops[j].mux
+                out_idxs[j] = len(ops_i)
+                ops_i.append([n + 2 * t, j, 6, n + 2 * t + 1])
+                ops_f.append([*ops[j].qint, max(q_out[j][3], q_out[n + 2 * t + 1][3]) + m[4], m[3]])
+            for j, a in enumerate(ops):
+                if a is not None and not isinstance(a, (_Mux, _View)):  # (the constant 0)
+                    out_idxs[j] = -1
+                elif q_out[j][0] == q_out[j][1] == 0.0 and not isinstance(a, _Mux):
+                    out_idxs[j] = -1
+            continue
         for j, a in enumerate(ops):
             if a is None:
                 continue
@@ -1626,11 +1772,8 @@ def _act_stage(layer, vals, k, seq, bias, a_sz, c_sz):
     for j, v in enumerate(nxt):
         if v[0] == v[1] == 0.0:
             out_idxs[j] = -1
-    st = dict(shape=(n, n), inp_shifts=np.zeros(n, np.int64), out_idxs=out_idxs, out_shifts=np.zeros(n, np.int64), out_negs=np.zeros(n, np.int64),
-              ops_i=np.asarray(ops_i, np.int64).reshape(-1, 4), ops_f=np.asarray(ops_f, np.float32).reshape(-1, 5), adder_size=a_sz, carry_size=c_sz)
-    if tables:
-        st['lookup_tables'] = tables
-    return st, nxt
+    close()
+    return stages, nxt
 
 
 PRICE_STATUS = ['ok', 'adder slower than the cutoff', 'not supported']  # PipelinePrice.status codes 0, 1, 2

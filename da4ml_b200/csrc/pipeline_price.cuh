@@ -35,10 +35,14 @@ enum PpStatus : int { PP_OK = 0, PP_SLOW_ADDER = 1 /* the tracer's AssertionErro
 // n1, which keeps its operand's latency (trace/fixed_variable.py:353-359, 381-384) and whose tracer cost is q0[0]; 4: a
 // constant addition of a constant (refused like 2, after the latency); 5: a lookup (opcode 8) of node n0 == n1, whose
 // latency is its operand's plus q0[1] (max(b_in - 6, 1), no register-boundary rule: trace/fixed_variable.py:331-340) and
-// whose tracer cost is q0[0].
+// whose tracer cost is q0[0]; 6: an MSB mux (opcode +-6) of the data nodes n0 / n1 on the condition node nc, whose latency is
+// the largest of its three operands' plus q0[1] (cost_add's latency of its data operands; msb_mux is built with an
+// explicit latency, so no register-boundary rule: trace/fixed_variable.py:841-859) and whose tracer cost is q0[0].  nc is
+// -1 for every other flag.
 struct PpAdd {
     int node, n0, n1, flag;
     float q0[3], q1[3];
+    int nc;
 };
 
 // Device view of a prepared design.  Node ids: [0, n_in) the network inputs, n_in the constant zero, then the adders.
@@ -115,6 +119,12 @@ template <bool COST> __device__ __forceinline__ void pp_replay(const PpDesign &d
     for (int l = 0; l < d.n_levels; ++l) {
         for (int k = d.lvl_begin[l] + tid; k < d.lvl_begin[l + 1]; k += nt) {
             const PpAdd a = d.adds[k];
+            if (a.flag == 6) { // an MSB mux: no adder, no boundary rule
+                t.lat[a.node] = pp_add(fmax(fmax(t.lat[a.n0], t.lat[a.n1]), t.lat[a.nc]), (double)a.q0[1]);
+                if (COST)
+                    cost_out[a.node] = a.q0[0];
+                continue;
+            }
             if (a.flag >= 3) { // an activation, a constant addition or a lookup: no adder
                 t.lat[a.node] = a.flag == 5 ? pp_add((double)a.q0[1], t.lat[a.n0]) : t.lat[a.n0];
                 if (COST)
@@ -193,6 +203,8 @@ __global__ void __launch_bounds__(256) pipeline_price_kernel(const PpDesign *des
         const int s = pp_stage(t.lat[a.node], c);
         atomicMax(&t.last_use[a.n0], s);
         atomicMax(&t.last_use[a.n1], s);
+        if (a.flag == 6)
+            atomicMax(&t.last_use[a.nc], s);
     }
     for (int o = tid; o < d.n_out; o += nt)
         atomicMax(&t.last_use[d.out_node[o]], s_out);
@@ -250,9 +262,12 @@ struct PpSplitInfo {
     std::vector<int> x, y, opc, data;   // per adder node - n_in - 1: FixedVariable.__add__'s operand order (the operand
                                         // with a positive factor first) and the op it becomes: opcode = (factor of y < 0),
                                         // data = log2|factor of y / factor of x|; an activation: x its operand, y -1,
-                                        // opcode +-2 / +-3 by the sign of the operand's factor, data 0
-    std::vector<double> xv, yv;         // per adder node - n_in - 1: the views x and y themselves, (lo, hi, step, factor)
-                                        // (y: zeros for an activation)
+                                        // opcode +-2 / +-3 by the sign of the operand's factor, data 0; an MSB mux: x / y
+                                        // its data operands a / b, opcode 6 or -6 by the sign of b's factor, data
+                                        // log2|factor of b / factor of a|
+    std::vector<int> z;                 // per adder node - n_in - 1: an MSB mux's condition node, else -1
+    std::vector<double> xv, yv, zv;     // per adder node - n_in - 1: the views x, y and z themselves, (lo, hi, step,
+                                        // factor) (y: zeros for an activation; z: zeros but for an MSB mux)
     std::vector<double> out_v;          // [n_out][4] each output's view
     std::vector<int64_t> out_shift;     // [n_out] log2|factor| of each output's view
     std::vector<char> out_neg;          // [n_out] factor < 0
@@ -388,24 +403,30 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
             // latency depend on intervals only), so the caller checks the index against them: the Python host does
             // (_design_tables), and a direct C ABI caller must.
             const bool lut = o[2] == 8;
+            // an MSB mux: data = shift << 32 | the condition's op (types.py:272-281)
+            const bool mux = o[2] == 6 || o[2] == -6;
+            const int64_t mux_c = o[3] & 0xffffffffll;
+            const int32_t mux_sh = (int32_t)(uint32_t)((uint64_t)o[3] >> 32);
             const bool ok = o[2] == -1 ? (o[0] >= 0 && o[0] < S.n_in && std::abs(S.inp_shifts[o[0]]) <= 512)
                             : (o[2] == 0 || o[2] == 1) ? (o[0] >= 0 && o[0] < i && o[1] >= 0 && o[1] < i && std::abs(o[3]) <= 512)
                             : act  ? (o[0] >= 0 && o[0] < i && o[1] == -1 && o[3] == 0)
                             : cadd ? (o[0] >= 0 && o[0] < i && o[1] == -1 && o[3] != 0 && std::llabs(o[3]) < (1ll << 31))
                             : lut  ? (o[0] >= 0 && o[0] < i && o[1] == -1 && o[3] >= 0 && o[3] < (1ll << 31))
+                            : mux  ? (o[0] >= 0 && o[0] < i && o[1] >= 0 && o[1] < i && mux_c < i && std::abs(mux_sh) <= 512)
                                    : false;
             if (!ok)
                 bad("stage " + std::to_string(s) + " op " + std::to_string(i) + ": opcode " + std::to_string(o[2]) + " with operands (" + std::to_string(o[0]) + ", " +
                     std::to_string(o[1]) + ") and data " + std::to_string(o[3]) + " is not an adder-graph op (opcodes -1, 0, 1, the activations +-2, +-3 "
-                    "and the constant addition 4 with 0 < |data| < 2^31, the lookup 8 with a table index; operands earlier ops, inputs in range)");
-            if (act || cadd || lut) { // the op's interval gives the activation's (k, i, f): a finite interval on a power-of-two grid
+                    "and the constant addition 4 with 0 < |data| < 2^31, the lookup 8 with a table index, the MSB mux +-6 with data shift << 32 | "
+                    "condition; operands earlier ops, inputs in range)");
+            if (act || cadd || lut || mux) { // the op's interval gives the activation's (k, i, f): a finite interval on a power-of-two grid
                 const float *q = S.ops_f + 5 * i;
                 const double lo = q[0], hi = q[1], st = q[2];
                 int e = 0;
                 const bool grid = std::isfinite(lo) && std::isfinite(hi) && st > 0 && std::isfinite(st) && std::frexp(st, &e) == 0.5 && lo <= hi &&
                                   std::fabs(lo / st) < 9.0e15 && std::fabs(hi / st) < 9.0e15 && lo / st == std::trunc(lo / st) && hi / st == std::trunc(hi / st);
                 if (!grid)
-                    bad("stage " + std::to_string(s) + " op " + std::to_string(i) + ": the interval of an " + (act ? "activation" : cadd ? "opcode 4 constant addition" : "opcode 8 lookup") +
+                    bad("stage " + std::to_string(s) + " op " + std::to_string(i) + ": the interval of an " + (act ? "activation" : cadd ? "opcode 4 constant addition" : lut ? "opcode 8 lookup" : "opcode +-6 MSB mux") +
                         " is not a quantized interval (min <= max, multiples of a power-of-two step)");
             }
         }
@@ -430,6 +451,7 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
         cur[k] = in_q[3 * k] == in_q[3 * k + 1] ? View{CONST, in_q[3 * k], in_q[3 * k + 1], in_q[3 * k + 2], 1.0} : view_of(k);
     std::vector<int> lvl(P.n_in + 1, 0);
     std::vector<char> is_cadd(P.n_in + 1, 0); // per node: a constant addition (FixedVariable.opr == 'cadd')
+    std::vector<char> is_wrap(P.n_in + 1, 0); // per node: a quantize (FixedVariable.opr == 'wrap')
     std::vector<PpAdd> adds;
     for (int64_t s = 0; s < n_stages; ++s) {
         const PpStageIn &S = st[s];
@@ -444,6 +466,7 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
                 const View V = buf[o[0]];
                 const double bias = (double)o[3] * (double)S.ops_f[5 * i + 2];
                 PpAdd a{};
+                a.nc = -1;
                 a.node = P.n_in + 1 + (int)adds.size();
                 a.n0 = a.n1 = V.node;
                 a.flag = 3;
@@ -461,8 +484,10 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
                 if (split) {
                     split->xv.insert(split->xv.end(), {V.lo, V.hi, V.step, V.f});
                     split->yv.insert(split->yv.end(), {0.0, 0.0, 0.0, 0.0});
+                    split->zv.insert(split->zv.end(), {0.0, 0.0, 0.0, 0.0});
                     split->x.push_back(V.node);
                     split->y.push_back(-1);
+                    split->z.push_back(-1);
                     split->opc.push_back(4);
                     // int(_data / unscaled step): the same through every view of the node
                     split->data.push_back((int)std::llround(d / (R.step / std::fabs(V.f))));
@@ -470,8 +495,63 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
                 node_view.push_back(R);
                 lvl.push_back(1 + lvl[V.node]);
                 is_cadd.push_back(1);
+                is_wrap.push_back(0);
                 adds.push_back(a);
                 buf[i] = R;
+                continue;
+            }
+            if (o[2] == 6 || o[2] == -6) { // CombLogic.__call__: k.msb_mux(v0, +-v1 * 2^shift, op.qint) (types.py:272-281)
+                const View K = buf[o[3] & 0xffffffffll];
+                View A = buf[o[0]], B = o[2] < 0 ? negated(buf[o[1]]) : buf[o[1]];
+                B = scaled(B, std::ldexp(1.0, (int32_t)(uint32_t)((uint64_t)o[3] >> 32)));
+                const std::string at = "stage " + std::to_string(s) + " op " + std::to_string(i) + ": an opcode +-6 MSB mux ";
+                if (K.lo == K.hi || A.lo == A.hi || B.lo == B.hi)
+                    bad(at + "with a constant operand (not covered)");
+                if (!(K.f > 0)) // (trace/tracer.py:119 asserts it of every traced mux)
+                    bad(at + "whose condition has a negative factor (the tracer asserts a positive one)");
+                if (is_wrap[K.node])
+                    bad(at + "whose condition is a quantize (the tracer may mux on its operand instead; not covered)");
+                // FixedVariable.msb_mux (trace/fixed_variable.py:788-859) with the explicit qint: a negative factor of a
+                // mirrors the qint and muxes -a, -b, seen negated
+                const float *q = S.ops_f + 5 * i;
+                double qlo = q[0], qhi = q[1];
+                const bool neg = A.f < 0;
+                if (neg) {
+                    const double t0 = 0.0 - qhi;
+                    qhi = 0.0 - qlo, qlo = t0;
+                    A = negated(A), B = negated(B);
+                }
+                const double step = std::min(A.step, B.step);
+                if (!((double)q[2] <= step))
+                    bad(at + "whose interval's step is larger than its operands' (the tracer asserts it is not)");
+                const double lo = std::max((std::floor(qlo / step) + 0.0) * step, std::min(A.lo, B.lo));
+                const double hi = std::min((std::floor(qhi / step) + 0.0) * step, std::max(A.hi, B.hi));
+                PpAdd a{};
+                a.node = P.n_in + 1 + (int)adds.size();
+                a.n0 = A.node;
+                a.n1 = B.node;
+                a.nc = K.node;
+                a.flag = 6;
+                float dl = 0.f, cost = 0.f;
+                cost_add(QInt{(float)A.lo, (float)A.hi, (float)A.step}, QInt{(float)B.lo, (float)B.hi, (float)B.step}, 0, false, P.adder_size, P.carry_size, dl, cost);
+                a.q0[0] = cost / 2.f;
+                a.q0[1] = dl;
+                if (split) {
+                    split->xv.insert(split->xv.end(), {A.lo, A.hi, A.step, A.f});
+                    split->yv.insert(split->yv.end(), {B.lo, B.hi, B.step, B.f});
+                    split->zv.insert(split->zv.end(), {K.lo, K.hi, K.step, K.f});
+                    split->x.push_back(A.node);
+                    split->y.push_back(B.node);
+                    split->z.push_back(K.node);
+                    split->opc.push_back(B.f > 0 ? 6 : -6);
+                    split->data.push_back((int)std::log2(std::fabs(B.f / A.f)));
+                }
+                node_view.push_back(View{a.node, lo, hi, step, A.f});
+                lvl.push_back(1 + std::max(std::max(lvl[A.node], lvl[B.node]), lvl[K.node]));
+                is_cadd.push_back(0);
+                is_wrap.push_back(0);
+                adds.push_back(a);
+                buf[i] = neg ? negated(node_view.back()) : node_view.back();
                 continue;
             }
             if (o[2] == 8) { // FixedVariable.lookup of the operand (CombLogic.__call__): the table's interval, factor 1
@@ -480,6 +560,7 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
                     bad("stage " + std::to_string(s) + " op " + std::to_string(i) + ": an opcode 8 lookup of a constant (the tracer makes a constant of it; not covered)");
                 const float *q = S.ops_f + 5 * i;
                 PpAdd a{};
+                a.nc = -1;
                 a.node = P.n_in + 1 + (int)adds.size();
                 a.n0 = a.n1 = V.node;
                 a.flag = 5;
@@ -493,14 +574,17 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
                 if (split) {
                     split->xv.insert(split->xv.end(), {V.lo, V.hi, V.step, V.f});
                     split->yv.insert(split->yv.end(), {0.0, 0.0, 0.0, 0.0});
+                    split->zv.insert(split->zv.end(), {0.0, 0.0, 0.0, 0.0});
                     split->x.push_back(V.node);
                     split->y.push_back(-1);
+                    split->z.push_back(-1);
                     split->opc.push_back(8);
                     split->data.push_back((int)o[3]);
                 }
                 node_view.push_back(View{a.node, (double)q[0], (double)q[1], (double)q[2], 1.0});
                 lvl.push_back(1 + lvl[V.node]);
                 is_cadd.push_back(0);
+                is_wrap.push_back(0);
                 adds.push_back(a);
                 buf[i] = node_view.back();
                 continue;
@@ -531,6 +615,7 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
                     continue;
                 }
                 PpAdd a{};
+                a.nc = -1;
                 a.node = P.n_in + 1 + (int)adds.size();
                 a.n0 = a.n1 = V.node;
                 a.flag = 3;
@@ -539,14 +624,17 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
                 if (split) {
                     split->xv.insert(split->xv.end(), {V.lo, V.hi, V.step, V.f});
                     split->yv.insert(split->yv.end(), {0.0, 0.0, 0.0, 0.0});
+                    split->zv.insert(split->zv.end(), {0.0, 0.0, 0.0, 0.0});
                     split->x.push_back(V.node);
                     split->y.push_back(-1);
+                    split->z.push_back(-1);
                     split->opc.push_back((V.f < 0 ? -1 : 1) * (relu ? 2 : 3));
                     split->data.push_back(0);
                 }
                 node_view.push_back(View{a.node, r.lo, r.hi, r.step, std::fabs(V.f)});
                 lvl.push_back(1 + lvl[V.node]);
                 is_cadd.push_back(0);
+                is_wrap.push_back(!relu);
                 adds.push_back(a);
                 buf[i] = node_view.back();
                 continue;
@@ -555,6 +643,7 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
             if (o[2] == 1)
                 B = negated(B);
             PpAdd a{};
+            a.nc = -1;
             a.node = P.n_in + 1 + (int)adds.size();
             a.n0 = A.node;
             a.n1 = B.node;
@@ -576,8 +665,10 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
             if (split) {
                 split->xv.insert(split->xv.end(), {X.lo, X.hi, X.step, X.f});
                 split->yv.insert(split->yv.end(), {Y.lo, Y.hi, Y.step, Y.f});
+                split->zv.insert(split->zv.end(), {0.0, 0.0, 0.0, 0.0});
                 split->x.push_back(X.node);
                 split->y.push_back(Y.node);
+                split->z.push_back(-1);
                 split->opc.push_back(Y.f < 0);
                 split->data.push_back((int)std::log2(std::fabs(Y.f / X.f)));
             }
@@ -586,6 +677,7 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
             node_view.push_back(View{a.node, lo, hi, step, f});
             lvl.push_back(1 + std::max(lvl[A.node], lvl[B.node]));
             is_cadd.push_back(0);
+            is_wrap.push_back(0);
             adds.push_back(a);
             buf[i] = node_view.back();
         }
@@ -622,8 +714,11 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
         P.out_bits += v.node == CONST ? 0 : pp_kif_bits(v.lo, v.hi, v.step);
     }
     for (size_t k = adds.size(); k-- > 0;)
-        if (live[adds[k].node])
+        if (live[adds[k].node]) {
             live[adds[k].n0] = live[adds[k].n1] = 1;
+            if (adds[k].nc >= 0)
+                live[adds[k].nc] = 1;
+        }
     P.node_bits.assign(P.n_nodes, -1);
     for (int v = 0; v < P.n_nodes; ++v) {
         if (!live[v])

@@ -15,7 +15,8 @@
 //                                the rows and outputs of every stage.  A stage with
 //                                no row or (before the last) no output is to_pipeline's KeyError, reported per task.
 //   pipeline_split_write_kernel  finds for every copy (a value carried across boundary j) the first event that needs it
-//                                (events: (op, operand 0 / operand 1 / the op itself), then the outputs), orders every
+//                                (events: (op, operand 0 / operand 1 / a mux's condition / the op itself), then the
+//                                outputs, the order of to_pipeline's _get_new_idx calls), orders every
 //                                stage's rows by the event that created them (a second radix sort over (stage, event)),
 //                                and writes the op tables with operands remapped to the reading stage's rows.
 // ps_split drives both, between them one small copy of the counts; the tables come back in one copy.
@@ -30,11 +31,15 @@ enum PsStatus : int { PS_SPLIT = 0, PS_NOT_OK = 1 /* the task is not ok: no spli
 
 struct PsItem {
     double lo, hi, step;  // the op's interval (the node's own)
+    long long data;       // see x, y, z, opc
     int node, gpos;       // node id (PpDesign) and position in gather_variables' list
-    int inp;              // >= 0: network input k; -1: adder; -2: constant (an all-zero output column); -3: activation
-    int x, y, opc, data;  // adder: items of the operands in _from order, opcode, shift; activation: the operand's item, y
-                          // -1, opcode +-2 / +-3, data 0; input: opcode -1, or 5 and the value in steps for an input with
-                          // a point interval (a constant to the tracer)
+    int inp;              // >= 0: network input k; -1: adder; -2: constant (an all-zero output column); -3: activation;
+                          // -4: MSB mux
+    int x, y, z, opc;     // adder: items of the operands in _from order, opcode, data the shift; activation: the operand's
+                          // item, y -1, opcode +-2 / +-3, data 0; MSB mux: the data operands a, b and the condition z
+                          // (_from is (z, a, b)), opcode +-6, data the shift of b (the written op's data is shift << 32 |
+                          // the condition's row); input: opcode -1, or 5 and the value in steps for an input with a point
+                          // interval (a constant to the tracer).  z is -1 but for a mux.
     int live;             // reachable from the outputs
 };
 
@@ -203,10 +208,12 @@ __global__ void __launch_bounds__(256) pipeline_split_kernel(const PsDesign *des
     // last consumer stage of every item: the stage of each adder reading it, and the output stage
     for (int i = tid; i < M; i += nt) {
         const PsItem &it = D.items[i];
-        if (it.inp == -1 || it.inp == -3)
+        if (it.inp == -1 || it.inp == -3 || it.inp == -4)
             atomicMax(&t.last[it.x], t.stg[i]);
-        if (it.inp == -1)
+        if (it.inp == -1 || it.inp == -4)
             atomicMax(&t.last[it.y], t.stg[i]);
+        if (it.inp == -4)
+            atomicMax(&t.last[it.z], t.stg[i]);
     }
     for (int o = tid; o < d.n_out; o += nt)
         atomicMax(&t.last[D.out_item[o]], s_out);
@@ -252,7 +259,7 @@ __global__ void __launch_bounds__(256) pipeline_split_write_kernel(const PsDesig
     const PsDesign D = designs[t.pp.design];
     const PsCount k0 = *t.count;
     const int tid = threadIdx.x, nt = blockDim.x, M = D.n_items, C = k0.n_copies, R = k0.n_kept + C, s_out = k0.s_out, n_out = D.pp.n_out;
-    const long long E = 3ll * M + n_out; // events: 3 * (op position) + (0, 1: its operands; 2: the op), then 3M + output
+    const long long E = 4ll * M + n_out; // events: 4 * (op position) + (0, 1: its operands; 2: a mux's condition; 3: the op), then 4M + output
     const double c = t.pp.cutoff;
     const int *stg = t.stg, *coff = t.coff, *rank = t.rank;
     for (int i = tid; i < M; i += nt)
@@ -263,28 +270,30 @@ __global__ void __launch_bounds__(256) pipeline_split_write_kernel(const PsDesig
     // across every boundary below s: record it at the last one, a suffix min then gives each copy its first event
     for (int i = tid; i < M; i += nt) {
         const PsItem &it = D.items[i];
-        if (it.inp != -1 && it.inp != -3)
+        if (it.inp != -1 && it.inp != -3 && it.inp != -4)
             continue;
         const int s = stg[i];
         if (s > stg[it.x])
-            atomicMin(&t.ev[coff[it.x] + s - 1 - stg[it.x]], 3 * rank[i]);
-        if (it.inp == -1 && s > stg[it.y])
-            atomicMin(&t.ev[coff[it.y] + s - 1 - stg[it.y]], 3 * rank[i] + 1);
+            atomicMin(&t.ev[coff[it.x] + s - 1 - stg[it.x]], 4 * rank[i]);
+        if (it.inp != -3 && s > stg[it.y])
+            atomicMin(&t.ev[coff[it.y] + s - 1 - stg[it.y]], 4 * rank[i] + 1);
+        if (it.inp == -4 && s > stg[it.z])
+            atomicMin(&t.ev[coff[it.z] + s - 1 - stg[it.z]], 4 * rank[i] + 2);
     }
     for (int o = tid; o < n_out; o += nt) {
         const int v = D.out_item[o];
         if (s_out > stg[v])
-            atomicMin(&t.ev[coff[v] + s_out - 1 - stg[v]], 3 * M + o);
+            atomicMin(&t.ev[coff[v] + s_out - 1 - stg[v]], 4 * M + o);
     }
     __syncthreads();
     for (int i = tid; i < M; i += nt)
         for (int k = coff[i + 1] - 2; k >= coff[i]; --k)
             t.ev[k] = min(t.ev[k], t.ev[k + 1]);
     __syncthreads();
-    // rows: the item's own (its stage, event 3p + 2) and its copies (stage j + 1, the copy's event); the R rows of the
+    // rows: the item's own (its stage, event 4p + 3) and its copies (stage j + 1, the copy's event); the R rows of the
     // split sort before the items that are not kept
     for (int i = tid; i < M; i += nt) {
-        t.rkey[i] = t.keep[i] ? (unsigned long long)stg[i] * E + 3ull * rank[i] + 2 : (unsigned long long)k0.n_st * E;
+        t.rkey[i] = t.keep[i] ? (unsigned long long)stg[i] * E + 4ull * rank[i] + 3 : (unsigned long long)k0.n_st * E;
         t.rval[i] = i;
     }
     for (int k = tid; k < C; k += nt) {
@@ -329,7 +338,9 @@ __global__ void __launch_bounds__(256) pipeline_split_write_kernel(const PsDesig
             else if (it.inp == -2)
                 oi[0] = -1, oi[1] = -1, oi[2] = 5, oi[3] = 0;
             else {
-                oi[0] = where(it.x, s), oi[1] = it.inp == -1 ? where(it.y, s) : -1, oi[2] = it.opc, oi[3] = it.data;
+                oi[0] = where(it.x, s), oi[1] = it.inp != -3 ? where(it.y, s) : -1, oi[2] = it.opc, oi[3] = it.data;
+                if (it.inp == -4) // to_pipeline's shift << 32 | the condition's row, the shift as its low 32 bits
+                    oi[3] = (int64_t)(((unsigned long long)(unsigned)it.data << 32) | (unsigned long long)where(it.z, s));
                 cost = (double)t.cost[it.node];
             }
             of[0] = it.lo, of[1] = it.hi, of[2] = it.step, of[3] = t.pp.lat[it.node], of[4] = cost;
@@ -358,7 +369,8 @@ struct PsPrep {
 };
 
 // gather_variables on the prepared design: every input at its position, then a depth-first post-order from the outputs
-// in output order, operands in _from order; the items are the gathered values dead_statement_elimination keeps.
+// in output order, operands in _from order (an MSB mux's condition first); the items are the gathered values
+// dead_statement_elimination keeps, which treats a mux's condition as a third operand.
 inline PsPrep ps_prepare(const PpPrepared &P, const PpSplitInfo &S) {
     PsPrep Q;
     const int CONST = P.n_in;
@@ -375,7 +387,7 @@ inline PsPrep ps_prepare(const PpPrepared &P, const PpSplitInfo &S) {
         it.node = node, it.gpos = gpos;
         it.lo = own[3 * (size_t)node], it.hi = own[3 * (size_t)node + 1], it.step = own[3 * (size_t)node + 2];
         it.inp = node < P.n_in ? node : node == CONST ? -2 : -1;
-        it.x = it.y = -1;
+        it.x = it.y = it.z = -1;
         it.opc = -1;
         it.live = node < P.n_in ? P.node_bits[node] >= 0 : 1;
         if (it.inp >= 0 && it.lo == it.hi) { // (0, 0, 2^32) for 0, else the step _const_f gives the value
@@ -398,6 +410,8 @@ inline PsPrep ps_prepare(const PpPrepared &P, const PpSplitInfo &S) {
             it.opc = S.opc[a], it.data = S.data[a];
             if (S.y[a] < 0) // relu / quantize
                 it.inp = -3;
+            if (S.z[a] >= 0) // an MSB mux
+                it.inp = -4, it.z = item_of[S.z[a]];
         }
         Q.items.push_back(it);
         return (int)Q.items.size() - 1;
@@ -445,6 +459,8 @@ inline PsPrep ps_prepare(const PpPrepared &P, const PpSplitInfo &S) {
                 if (S.y[a] >= 0)
                     stack.push_back({S.y[a], false, S.yv.data() + 4 * (size_t)a});
                 stack.push_back({S.x[a], false, S.xv.data() + 4 * (size_t)a});
+                if (S.z[a] >= 0) // an MSB mux's _from is (condition, a, b)
+                    stack.push_back({S.z[a], false, S.zv.data() + 4 * (size_t)a});
             }
         }
         Q.out_item.push_back(item_of[root]);
