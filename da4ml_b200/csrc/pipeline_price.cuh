@@ -28,19 +28,30 @@ namespace da {
 
 enum PpStatus : int { PP_OK = 0, PP_SLOW_ADDER = 1 /* the tracer's AssertionError */, PP_UNSUPPORTED = 2 /* a constant intermediate value */ };
 
-// One adder of a design, in dependency-level order.  `node` is its own node id; n0 / n1 the nodes its operands view; q0 /
-// q1 the operand intervals cost_add receives (after FixedVariable.__add__'s sign normalisation, as float32); `flag` 2: an
-// operand is a constant (refused before the latency), 1: the sum is a constant (refused after the latency), 0: neither;
-// 3: not an adder but an activation (relu / quantize, opcodes +-2 / +-3) or a constant addition (opcode 4) of node n0 ==
-// n1, which keeps its operand's latency (trace/fixed_variable.py:353-359, 381-384) and whose tracer cost is q0[0]; 4: a
-// constant addition of a constant (refused like 2, after the latency); 5: a lookup (opcode 8) of node n0 == n1, whose
-// latency is its operand's plus q0[1] (max(b_in - 6, 1), no register-boundary rule: trace/fixed_variable.py:331-340) and
-// whose tracer cost is q0[0]; 6: an MSB mux (opcode +-6) of the data nodes n0 / n1 on the condition node nc, whose latency is
-// the largest of its three operands' plus q0[1] (cost_add's latency of its data operands; msb_mux is built with an
-// explicit latency, so no register-boundary rule: trace/fixed_variable.py:841-859) and whose tracer cost is q0[0].  nc is
-// -1 for every other flag.
+// What the node of a PpAdd is.  The order matters: no flag from PP_ONE_OPERAND on is an adder (no cost_add, no
+// register-boundary rule), and pp_replay tests that as `flag >= PP_ONE_OPERAND`.
+enum PpFlag : int {
+    PP_ADDER = 0,          // an adder
+    PP_CONST_SUM = 1,      // an adder whose sum is a constant (refused after the latency)
+    PP_CONST_OPERAND = 2,  // an adder with a constant operand (refused before the latency)
+    PP_ONE_OPERAND = 3,    // an activation (relu / quantize, opcodes +-2 / +-3) or a constant addition (opcode 4) of
+                           // node n0 == n1: its operand's latency (trace/fixed_variable.py:353-359, 381-384); tracer
+                           // cost q0[0]
+    PP_CONST_CADD = 4,     // a constant addition of a constant (refused like PP_CONST_OPERAND, after the latency)
+    PP_LOOKUP = 5,         // a lookup (opcode 8) of node n0 == n1: its operand's latency plus q0[1] (max(b_in - 6, 1),
+                           // no register-boundary rule: trace/fixed_variable.py:331-340); tracer cost q0[0]
+    PP_MUX = 6,            // an MSB mux (opcode +-6) of the data nodes n0 / n1 on the condition node nc: the largest of
+                           // its three operands' latencies plus q0[1] (cost_add's latency of its data operands; msb_mux
+                           // is built with an explicit latency, so no register-boundary rule:
+                           // trace/fixed_variable.py:841-859); tracer cost q0[0]
+};
+
+// One node an op of a design creates, in dependency-level order.  `node` is its own node id; n0 / n1 the nodes its operands
+// view; for an adder, q0 / q1 the operand intervals cost_add receives (after FixedVariable.__add__'s sign normalisation, as
+// float32); nc the condition node of an MSB mux, -1 for every other flag.
 struct PpAdd {
-    int node, n0, n1, flag;
+    int node, n0, n1;
+    PpFlag flag;
     float q0[3], q1[3];
     int nc;
 };
@@ -119,17 +130,17 @@ template <bool COST> __device__ __forceinline__ void pp_replay(const PpDesign &d
     for (int l = 0; l < d.n_levels; ++l) {
         for (int k = d.lvl_begin[l] + tid; k < d.lvl_begin[l + 1]; k += nt) {
             const PpAdd a = d.adds[k];
-            if (a.flag == 6) { // an MSB mux: no adder, no boundary rule
+            if (a.flag == PP_MUX) { // no adder, no boundary rule
                 t.lat[a.node] = pp_add(fmax(fmax(t.lat[a.n0], t.lat[a.n1]), t.lat[a.nc]), (double)a.q0[1]);
                 if (COST)
                     cost_out[a.node] = a.q0[0];
                 continue;
             }
-            if (a.flag >= 3) { // an activation, a constant addition or a lookup: no adder
-                t.lat[a.node] = a.flag == 5 ? pp_add((double)a.q0[1], t.lat[a.n0]) : t.lat[a.n0];
+            if (a.flag >= PP_ONE_OPERAND) { // an activation, a constant addition or a lookup: no adder
+                t.lat[a.node] = a.flag == PP_LOOKUP ? pp_add((double)a.q0[1], t.lat[a.n0]) : t.lat[a.n0];
                 if (COST)
                     cost_out[a.node] = a.q0[0];
-                if (a.flag == 4) // (of a constant)
+                if (a.flag == PP_CONST_CADD)
                     atomicMin(&s_fail, ((unsigned long long)a.node << 2) | (unsigned long long)PP_UNSUPPORTED);
                 continue;
             }
@@ -145,7 +156,7 @@ template <bool COST> __device__ __forceinline__ void pp_replay(const PpDesign &d
             t.lat[a.node] = lat;
             if (COST)
                 cost_out[a.node] = cost;
-            const int st = a.flag == 2 ? PP_UNSUPPORTED : slow ? PP_SLOW_ADDER : a.flag == 1 ? PP_UNSUPPORTED : PP_OK;
+            const int st = a.flag == PP_CONST_OPERAND ? PP_UNSUPPORTED : slow ? PP_SLOW_ADDER : a.flag == PP_CONST_SUM ? PP_UNSUPPORTED : PP_OK;
             if (st != PP_OK)
                 atomicMin(&s_fail, ((unsigned long long)a.node << 2) | (unsigned long long)st);
         }
@@ -203,7 +214,7 @@ __global__ void __launch_bounds__(256) pipeline_price_kernel(const PpDesign *des
         const int s = pp_stage(t.lat[a.node], c);
         atomicMax(&t.last_use[a.n0], s);
         atomicMax(&t.last_use[a.n1], s);
-        if (a.flag == 6)
+        if (a.flag == PP_MUX)
             atomicMax(&t.last_use[a.nc], s);
     }
     for (int o = tid; o < d.n_out; o += nt)
@@ -255,20 +266,29 @@ struct PpStageIn {
     const float *ops_f;                                                     // [n_ops][5]
 };
 
+// A node seen through a scaling: the interval of the scaled value and its factor (+-2^k).
+struct PpView {
+    int node;
+    double lo, hi, step, f;
+};
+
+// What a split needs of one node an op creates: its operands as views of their nodes, and the op it becomes.  An adder: x
+// and y in FixedVariable.__add__'s operand order (the operand with a positive factor first), opcode = (factor of y < 0),
+// data = log2|factor of y / factor of x|.  A one-operand op: x its operand, y none; relu / quantize: opcode +-2 / +-3 by
+// the sign of the operand's factor, data 0; a constant addition: opcode 4, data the addend in steps; a lookup: opcode 8,
+// data the table index.  An MSB mux: x / y its data operands a / b, opcode 6 or -6 by the sign of b's factor, data
+// log2|factor of b / factor of a|.  z is the mux's condition, none for every other op.  None: node -1, zeros.
+struct PpSplitOp {
+    PpView x, y, z;
+    int opc, data;
+};
+
 // What a split needs beyond pricing, recorded by pp_prepare only when asked for (pipeline_split.cuh).  Node ids as in
 // PpDesign; the constant node stands for every all-zero output column.
 struct PpSplitInfo {
     std::vector<double> own_q;          // [n_nodes][3] the node's own (unscaled) interval; the constant: (0, 0, 2^32)
-    std::vector<int> x, y, opc, data;   // per adder node - n_in - 1: FixedVariable.__add__'s operand order (the operand
-                                        // with a positive factor first) and the op it becomes: opcode = (factor of y < 0),
-                                        // data = log2|factor of y / factor of x|; an activation: x its operand, y -1,
-                                        // opcode +-2 / +-3 by the sign of the operand's factor, data 0; an MSB mux: x / y
-                                        // its data operands a / b, opcode 6 or -6 by the sign of b's factor, data
-                                        // log2|factor of b / factor of a|
-    std::vector<int> z;                 // per adder node - n_in - 1: an MSB mux's condition node, else -1
-    std::vector<double> xv, yv, zv;     // per adder node - n_in - 1: the views x, y and z themselves, (lo, hi, step,
-                                        // factor) (y: zeros for an activation; z: zeros but for an MSB mux)
-    std::vector<double> out_v;          // [n_out][4] each output's view
+    std::vector<PpSplitOp> ops;         // [node - n_in - 1] per node an op creates
+    std::vector<PpView> out_v;          // [n_out] each output's view
     std::vector<int64_t> out_shift;     // [n_out] log2|factor| of each output's view
     std::vector<char> out_neg;          // [n_out] factor < 0
 };
@@ -352,29 +372,21 @@ inline int pp_const_f(double c) {
     return hi;
 }
 
-// sum of minimal_kif (types.py:86-114) of an interval
+// sum of minimal_kif of an interval
 inline int pp_kif_bits(double lo, double hi, double step) {
-    if (lo == 0.0 && hi == 0.0)
-        return 0;
-    const int keep_neg = lo < 0;
-    const int frac = (int)(-std::log2(step));
-    const double imin = std::nearbyint(lo / step), imax = std::nearbyint(hi / step);
-    const int bits = (int)std::ceil(std::log2(std::max(std::fabs(imin), imax + 1)));
-    return keep_neg + bits;
+    int k, i, f;
+    pp_minimal_kif(lo, hi, step, k, i, f);
+    return k + i + f;
 }
 
 // Check one design's arrays (DA4ML_E_INVALID-class errors are thrown as std::invalid_argument) and prepare it.
 inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo *split = nullptr) {
-    struct View { // a node seen through a scaling: interval of the scaled value and its factor (+-2^k)
-        int node;
-        double lo, hi, step, f;
-    };
-    auto scaled = [](View v, double s) {
+    auto scaled = [](PpView v, double s) {
         const double a = v.lo * s, b = v.hi * s;
-        return View{v.node, std::min(a, b), std::max(a, b), std::fabs(v.step * s), v.f * s};
+        return PpView{v.node, std::min(a, b), std::max(a, b), std::fabs(v.step * s), v.f * s};
     };
     // FixedVariable.__neg__: Decimal negation, whose zero is +0 (a product with a negative power of two gives -0)
-    auto negated = [](View v) { return View{v.node, 0.0 - v.hi, 0.0 - v.lo, v.step, -v.f}; };
+    auto negated = [](PpView v) { return PpView{v.node, 0.0 - v.hi, 0.0 - v.lo, v.step, -v.f}; };
     auto bad = [](const std::string &m) { throw std::invalid_argument("pipeline_price: " + m); };
     if (n_stages < 1)
         bad("a design needs at least one stage");
@@ -383,10 +395,6 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
     P.adder_size = (int)st[0].adder_size;
     P.carry_size = (int)st[0].carry_size;
     const int CONST = P.n_in;
-    std::vector<View> node_view; // the view an adder node was created with
-    std::vector<double> in_q(3 * (size_t)P.n_in);
-    for (int k = 0; k < P.n_in; ++k)
-        in_q[3 * k] = 0.0, in_q[3 * k + 1] = 0.0, in_q[3 * k + 2] = 1.0;
     for (int64_t s = 0; s < n_stages; ++s) {
         const PpStageIn &S = st[s];
         if (S.n_in < 0 || S.n_out < 0 || S.n_ops < 0 || (s > 0 && S.n_in != st[s - 1].n_out))
@@ -434,28 +442,43 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
             if (S.out_idxs[k] < -1 || S.out_idxs[k] >= S.n_ops || std::abs(S.out_shifts[k]) > 512)
                 bad("stage " + std::to_string(s) + " output " + std::to_string(k) + " is out of range");
     }
+    struct Node {
+        PpView v;        // the view the node was created with
+        int lvl;         // dependency level: 0 for the inputs and the constant
+        bool cadd, wrap; // a constant addition / a quantize (FixedVariable.opr == 'cadd' / 'wrap')
+    };
+    std::vector<Node> nodes(P.n_in + 1); // indexed by node id
+    for (int k = 0; k < P.n_in; ++k)
+        nodes[k].v = PpView{k, 0.0, 0.0, 1.0, 1.0};
     for (int64_t i = 0; i < st[0].n_ops; ++i) // the design's input intervals (CombLogic.inp_qint)
-        if (st[0].ops_i[4 * i + 2] == -1)
-            for (int j = 0; j < 3; ++j)
-                in_q[3 * st[0].ops_i[4 * i] + j] = st[0].ops_f[5 * i + j];
-    auto view_of = [&](int node) -> View {
-        if (node == CONST)
-            return View{CONST, 0.0, 0.0, 4294967296.0, 1.0};
-        if (node < P.n_in)
-            return View{node, in_q[3 * node], in_q[3 * node + 1], in_q[3 * node + 2], 1.0};
-        return node_view[node - P.n_in - 1];
+        if (st[0].ops_i[4 * i + 2] == -1) {
+            const int k = (int)st[0].ops_i[4 * i];
+            const float *q = st[0].ops_f + 5 * i;
+            nodes[k].v = PpView{k, q[0], q[1], q[2], 1.0};
+        }
+    nodes[CONST].v = PpView{CONST, 0.0, 0.0, 4294967296.0, 1.0};
+    std::vector<PpAdd> adds;
+    const PpView none{-1, 0.0, 0.0, 0.0, 0.0};
+    // Record op `a` as the next node, created with view `v` (both get its id), with its level and split record; returns
+    // the view.  Node ids are the order of this call.
+    auto add_node = [&](PpAdd a, PpView v, const PpSplitOp &op, bool cadd = false, bool wrap = false) {
+        a.node = v.node = (int)nodes.size();
+        const int lvl = 1 + std::max(std::max(nodes[a.n0].lvl, nodes[a.n1].lvl), a.nc >= 0 ? nodes[a.nc].lvl : 0);
+        adds.push_back(a);
+        nodes.push_back(Node{v, lvl, cadd, wrap});
+        if (split)
+            split->ops.push_back(op);
+        return v;
     };
     // replay: cur = the views entering the stage
-    std::vector<View> cur(P.n_in);
-    for (int k = 0; k < P.n_in; ++k)
-        cur[k] = in_q[3 * k] == in_q[3 * k + 1] ? View{CONST, in_q[3 * k], in_q[3 * k + 1], in_q[3 * k + 2], 1.0} : view_of(k);
-    std::vector<int> lvl(P.n_in + 1, 0);
-    std::vector<char> is_cadd(P.n_in + 1, 0); // per node: a constant addition (FixedVariable.opr == 'cadd')
-    std::vector<char> is_wrap(P.n_in + 1, 0); // per node: a quantize (FixedVariable.opr == 'wrap')
-    std::vector<PpAdd> adds;
+    std::vector<PpView> cur(P.n_in);
+    for (int k = 0; k < P.n_in; ++k) {
+        const PpView &w = nodes[k].v;
+        cur[k] = w.lo == w.hi ? PpView{CONST, w.lo, w.hi, w.step, 1.0} : w;
+    }
     for (int64_t s = 0; s < n_stages; ++s) {
         const PpStageIn &S = st[s];
-        std::vector<View> buf(S.n_ops);
+        std::vector<PpView> buf(S.n_ops);
         for (int64_t i = 0; i < S.n_ops; ++i) {
             const int64_t *o = S.ops_i + 4 * i;
             if (o[2] == -1) {
@@ -463,53 +486,36 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
                 continue;
             }
             if (o[2] == 4) { // FixedVariable._const_add of data * step (CombLogic.__call__, types.py:267-269)
-                const View V = buf[o[0]];
+                const PpView V = buf[o[0]];
                 const double bias = (double)o[3] * (double)S.ops_f[5 * i + 2];
                 PpAdd a{};
-                a.nc = -1;
-                a.node = P.n_in + 1 + (int)adds.size();
-                a.n0 = a.n1 = V.node;
-                a.flag = 3;
-                View R{a.node, V.lo + bias, V.hi + bias, std::min(V.step, std::ldexp(1.0, -pp_const_f(bias))), V.f};
+                a.n0 = a.n1 = V.node, a.nc = -1;
+                a.flag = PP_ONE_OPERAND;
+                PpView R{-1, V.lo + bias, V.hi + bias, std::min(V.step, std::ldexp(1.0, -pp_const_f(bias))), V.f};
                 if (V.lo == V.hi) { // a constant plus a constant: not supported, as an adder of a constant is not
-                    a.flag = 4;
+                    a.flag = PP_CONST_CADD;
                     R.step = V.step;
-                } else if (is_cadd[V.node]) {
+                } else if (nodes[V.node].cadd) {
                     bad("stage " + std::to_string(s) + " op " + std::to_string(i) + ": an opcode 4 constant addition of a constant addition (the tracer folds "
                         "the two into one op on the earlier operand; not covered)");
                 }
                 const double d = bias / V.f; // the node's _data, and the tracer's cost ceil(log2(|d| + 2^-f)) + f
                 const int fd = pp_const_f(d);
                 a.q0[0] = (float)(std::ceil(std::log2(std::fabs(d) + std::ldexp(1.0, -fd))) + fd);
-                if (split) {
-                    split->xv.insert(split->xv.end(), {V.lo, V.hi, V.step, V.f});
-                    split->yv.insert(split->yv.end(), {0.0, 0.0, 0.0, 0.0});
-                    split->zv.insert(split->zv.end(), {0.0, 0.0, 0.0, 0.0});
-                    split->x.push_back(V.node);
-                    split->y.push_back(-1);
-                    split->z.push_back(-1);
-                    split->opc.push_back(4);
-                    // int(_data / unscaled step): the same through every view of the node
-                    split->data.push_back((int)std::llround(d / (R.step / std::fabs(V.f))));
-                }
-                node_view.push_back(R);
-                lvl.push_back(1 + lvl[V.node]);
-                is_cadd.push_back(1);
-                is_wrap.push_back(0);
-                adds.push_back(a);
-                buf[i] = R;
+                // data: int(_data / unscaled step), the same through every view of the node
+                buf[i] = add_node(a, R, PpSplitOp{V, none, none, 4, (int)std::llround(d / (R.step / std::fabs(V.f)))}, true);
                 continue;
             }
             if (o[2] == 6 || o[2] == -6) { // CombLogic.__call__: k.msb_mux(v0, +-v1 * 2^shift, op.qint) (types.py:272-281)
-                const View K = buf[o[3] & 0xffffffffll];
-                View A = buf[o[0]], B = o[2] < 0 ? negated(buf[o[1]]) : buf[o[1]];
+                const PpView K = buf[o[3] & 0xffffffffll];
+                PpView A = buf[o[0]], B = o[2] < 0 ? negated(buf[o[1]]) : buf[o[1]];
                 B = scaled(B, std::ldexp(1.0, (int32_t)(uint32_t)((uint64_t)o[3] >> 32)));
                 const std::string at = "stage " + std::to_string(s) + " op " + std::to_string(i) + ": an opcode +-6 MSB mux ";
                 if (K.lo == K.hi || A.lo == A.hi || B.lo == B.hi)
                     bad(at + "with a constant operand (not covered)");
                 if (!(K.f > 0)) // (trace/tracer.py:119 asserts it of every traced mux)
                     bad(at + "whose condition has a negative factor (the tracer asserts a positive one)");
-                if (is_wrap[K.node])
+                if (nodes[K.node].wrap)
                     bad(at + "whose condition is a quantize (the tracer may mux on its operand instead; not covered)");
                 // FixedVariable.msb_mux (trace/fixed_variable.py:788-859) with the explicit qint: a negative factor of a
                 // mirrors the qint and muxes -a, -b, seen negated
@@ -527,43 +533,24 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
                 const double lo = std::max((std::floor(qlo / step) + 0.0) * step, std::min(A.lo, B.lo));
                 const double hi = std::min((std::floor(qhi / step) + 0.0) * step, std::max(A.hi, B.hi));
                 PpAdd a{};
-                a.node = P.n_in + 1 + (int)adds.size();
-                a.n0 = A.node;
-                a.n1 = B.node;
-                a.nc = K.node;
-                a.flag = 6;
+                a.n0 = A.node, a.n1 = B.node, a.nc = K.node;
+                a.flag = PP_MUX;
                 float dl = 0.f, cost = 0.f;
                 cost_add(QInt{(float)A.lo, (float)A.hi, (float)A.step}, QInt{(float)B.lo, (float)B.hi, (float)B.step}, 0, false, P.adder_size, P.carry_size, dl, cost);
                 a.q0[0] = cost / 2.f;
                 a.q0[1] = dl;
-                if (split) {
-                    split->xv.insert(split->xv.end(), {A.lo, A.hi, A.step, A.f});
-                    split->yv.insert(split->yv.end(), {B.lo, B.hi, B.step, B.f});
-                    split->zv.insert(split->zv.end(), {K.lo, K.hi, K.step, K.f});
-                    split->x.push_back(A.node);
-                    split->y.push_back(B.node);
-                    split->z.push_back(K.node);
-                    split->opc.push_back(B.f > 0 ? 6 : -6);
-                    split->data.push_back((int)std::log2(std::fabs(B.f / A.f)));
-                }
-                node_view.push_back(View{a.node, lo, hi, step, A.f});
-                lvl.push_back(1 + std::max(std::max(lvl[A.node], lvl[B.node]), lvl[K.node]));
-                is_cadd.push_back(0);
-                is_wrap.push_back(0);
-                adds.push_back(a);
-                buf[i] = neg ? negated(node_view.back()) : node_view.back();
+                const PpView R = add_node(a, PpView{-1, lo, hi, step, A.f}, PpSplitOp{A, B, K, B.f > 0 ? 6 : -6, (int)std::log2(std::fabs(B.f / A.f))});
+                buf[i] = neg ? negated(R) : R;
                 continue;
             }
             if (o[2] == 8) { // FixedVariable.lookup of the operand (CombLogic.__call__): the table's interval, factor 1
-                const View V = buf[o[0]];
+                const PpView V = buf[o[0]];
                 if (V.lo == V.hi)
                     bad("stage " + std::to_string(s) + " op " + std::to_string(i) + ": an opcode 8 lookup of a constant (the tracer makes a constant of it; not covered)");
                 const float *q = S.ops_f + 5 * i;
                 PpAdd a{};
-                a.nc = -1;
-                a.node = P.n_in + 1 + (int)adds.size();
-                a.n0 = a.n1 = V.node;
-                a.flag = 5;
+                a.n0 = a.n1 = V.node, a.nc = -1;
+                a.flag = PP_LOOKUP;
                 // get_cost_and_latency: b_in the kif bits of the operand as the tracer sees it, b_out the result's
                 const int b_in = pp_kif_prop_bits(V.lo, V.hi, V.step), b_out = pp_kif_prop_bits(q[0], q[1], q[2]);
                 double cost = std::ldexp(1.0, std::max(b_in - 5, 0)) * std::ceil(b_out / 2.0);
@@ -571,31 +558,16 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
                     cost *= b_in / 5.0;
                 a.q0[0] = (float)cost;
                 a.q0[1] = (float)std::max(b_in - 6, 1);
-                if (split) {
-                    split->xv.insert(split->xv.end(), {V.lo, V.hi, V.step, V.f});
-                    split->yv.insert(split->yv.end(), {0.0, 0.0, 0.0, 0.0});
-                    split->zv.insert(split->zv.end(), {0.0, 0.0, 0.0, 0.0});
-                    split->x.push_back(V.node);
-                    split->y.push_back(-1);
-                    split->z.push_back(-1);
-                    split->opc.push_back(8);
-                    split->data.push_back((int)o[3]);
-                }
-                node_view.push_back(View{a.node, (double)q[0], (double)q[1], (double)q[2], 1.0});
-                lvl.push_back(1 + lvl[V.node]);
-                is_cadd.push_back(0);
-                is_wrap.push_back(0);
-                adds.push_back(a);
-                buf[i] = node_view.back();
+                buf[i] = add_node(a, PpView{-1, q[0], q[1], q[2], 1.0}, PpSplitOp{V, none, none, 8, (int)o[3]});
                 continue;
             }
             if (o[2] != 0 && o[2] != 1) { // relu (+-2) / quantize (+-3) of the operand (negated for the negative opcode)
-                View V = o[2] < 0 ? negated(buf[o[0]]) : buf[o[0]];
+                PpView V = o[2] < 0 ? negated(buf[o[0]]) : buf[o[0]];
                 if (V.lo == V.hi) { // a constant: the tracer folds it (relu / quantize of 0 is 0)
                     if (V.lo != 0.0)
                         bad("stage " + std::to_string(s) + " op " + std::to_string(i) + ": an activation of the constant " + std::to_string(V.lo) +
                             " (only the constant 0 is covered)");
-                    buf[i] = view_of(CONST);
+                    buf[i] = nodes[CONST].v;
                     continue;
                 }
                 const float *q = S.ops_f + 5 * i;
@@ -611,44 +583,24 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
                     if (r.lo != 0.0)
                         bad("stage " + std::to_string(s) + " op " + std::to_string(i) + ": the activation makes the constant " + std::to_string(r.lo) +
                             " (only the constant 0 is covered)");
-                    buf[i] = view_of(CONST);
+                    buf[i] = nodes[CONST].v;
                     continue;
                 }
                 PpAdd a{};
-                a.nc = -1;
-                a.node = P.n_in + 1 + (int)adds.size();
-                a.n0 = a.n1 = V.node;
-                a.flag = 3;
+                a.n0 = a.n1 = V.node, a.nc = -1;
+                a.flag = PP_ONE_OPERAND;
                 const int kb = pp_kif_prop_bits(r.lo, r.hi, r.step); // the tracer's cost: half a LUT per bit for relu, and for a negation
                 a.q0[0] = (float)((V.f < 0 ? kb / 2.0 : 0.0) + (relu ? kb / 2.0 : 0.0));
-                if (split) {
-                    split->xv.insert(split->xv.end(), {V.lo, V.hi, V.step, V.f});
-                    split->yv.insert(split->yv.end(), {0.0, 0.0, 0.0, 0.0});
-                    split->zv.insert(split->zv.end(), {0.0, 0.0, 0.0, 0.0});
-                    split->x.push_back(V.node);
-                    split->y.push_back(-1);
-                    split->z.push_back(-1);
-                    split->opc.push_back((V.f < 0 ? -1 : 1) * (relu ? 2 : 3));
-                    split->data.push_back(0);
-                }
-                node_view.push_back(View{a.node, r.lo, r.hi, r.step, std::fabs(V.f)});
-                lvl.push_back(1 + lvl[V.node]);
-                is_cadd.push_back(0);
-                is_wrap.push_back(!relu);
-                adds.push_back(a);
-                buf[i] = node_view.back();
+                buf[i] = add_node(a, PpView{-1, r.lo, r.hi, r.step, std::fabs(V.f)}, PpSplitOp{V, none, none, (V.f < 0 ? -1 : 1) * (relu ? 2 : 3), 0}, false, !relu);
                 continue;
             }
-            View A = buf[o[0]], B = scaled(buf[o[1]], std::ldexp(1.0, (int)o[3]));
+            PpView A = buf[o[0]], B = scaled(buf[o[1]], std::ldexp(1.0, (int)o[3]));
             if (o[2] == 1)
                 B = negated(B);
             PpAdd a{};
-            a.nc = -1;
-            a.node = P.n_in + 1 + (int)adds.size();
-            a.n0 = A.node;
-            a.n1 = B.node;
-            a.flag = (A.lo == A.hi || B.lo == B.hi) ? 2 : 0;
-            View X = A, Y = B; // FixedVariable.__add__: the operand with a positive factor first; both negative: negate both
+            a.n0 = A.node, a.n1 = B.node, a.nc = -1;
+            a.flag = (A.lo == A.hi || B.lo == B.hi) ? PP_CONST_OPERAND : PP_ADDER;
+            PpView X = A, Y = B; // FixedVariable.__add__: the operand with a positive factor first; both negative: negate both
             bool neg = false;
             if (A.f < 0) {
                 if (B.f > 0)
@@ -662,53 +614,37 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
             const double lo = neg ? 0.0 - chi : clo, hi = neg ? 0.0 - clo : chi, f = neg ? -X.f : X.f;
             a.q0[0] = (float)X.lo, a.q0[1] = (float)X.hi, a.q0[2] = (float)X.step;
             a.q1[0] = (float)Y.lo, a.q1[1] = (float)Y.hi, a.q1[2] = (float)Y.step;
-            if (split) {
-                split->xv.insert(split->xv.end(), {X.lo, X.hi, X.step, X.f});
-                split->yv.insert(split->yv.end(), {Y.lo, Y.hi, Y.step, Y.f});
-                split->zv.insert(split->zv.end(), {0.0, 0.0, 0.0, 0.0});
-                split->x.push_back(X.node);
-                split->y.push_back(Y.node);
-                split->z.push_back(-1);
-                split->opc.push_back(Y.f < 0);
-                split->data.push_back((int)std::log2(std::fabs(Y.f / X.f)));
-            }
-            if (a.flag == 0 && lo == hi)
-                a.flag = 1;
-            node_view.push_back(View{a.node, lo, hi, step, f});
-            lvl.push_back(1 + std::max(lvl[A.node], lvl[B.node]));
-            is_cadd.push_back(0);
-            is_wrap.push_back(0);
-            adds.push_back(a);
-            buf[i] = node_view.back();
+            if (a.flag == PP_ADDER && lo == hi)
+                a.flag = PP_CONST_SUM;
+            buf[i] = add_node(a, PpView{-1, lo, hi, step, f}, PpSplitOp{X, Y, none, Y.f < 0, (int)std::log2(std::fabs(Y.f / X.f))});
         }
-        std::vector<View> next(S.n_out);
+        std::vector<PpView> next(S.n_out);
         for (int64_t k = 0; k < S.n_out; ++k) {
             const int64_t i = S.out_idxs[k];
             if (i < 0)
-                next[k] = view_of(CONST);
+                next[k] = nodes[CONST].v;
             else
                 next[k] = scaled(scaled(buf[i], std::ldexp(1.0, (int)S.out_shifts[k])), S.out_negs[k] ? -1.0 : 1.0);
         }
         cur.swap(next);
     }
-    P.n_nodes = P.n_in + 1 + (int)adds.size();
+    P.n_nodes = (int)nodes.size();
     P.n_out = (int)cur.size();
     if (split) {
         split->own_q.resize(3 * (size_t)P.n_nodes);
         for (int v = 0; v < P.n_nodes; ++v) {
-            View w = view_of(v);
-            w = scaled(w, 1.0 / w.f); // FixedVariable.unscaled
+            const PpView w = scaled(nodes[v].v, 1.0 / nodes[v].v.f); // FixedVariable.unscaled
             split->own_q[3 * v] = w.lo, split->own_q[3 * v + 1] = w.hi, split->own_q[3 * v + 2] = w.step;
         }
-        for (const View &v : cur) {
-            split->out_v.insert(split->out_v.end(), {v.lo, v.hi, v.step, v.f});
+        split->out_v = cur;
+        for (const PpView &v : cur) {
             split->out_shift.push_back((int64_t)std::log2(std::fabs(v.f)));
             split->out_neg.push_back(v.f < 0);
         }
     }
     // liveness (comb_trace's dead-statement elimination) and bits
     std::vector<char> live(P.n_nodes, 0);
-    for (const View &v : cur) {
+    for (const PpView &v : cur) {
         P.out_node.push_back(v.node);
         live[v.node] = 1;
         P.out_bits += v.node == CONST ? 0 : pp_kif_bits(v.lo, v.hi, v.step);
@@ -727,7 +663,7 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
             P.node_bits[v] = 0;
             continue;
         }
-        View w = view_of(v);
+        PpView w = nodes[v].v;
         if (w.f < 0)
             w = scaled(w, -1.0); // the node's own interval (the op's qint in the traced graph)
         P.node_bits[v] = pp_kif_bits(w.lo, w.hi, w.step);
@@ -735,16 +671,16 @@ inline PpPrepared pp_prepare(const PpStageIn *st, int64_t n_stages, PpSplitInfo 
     // adders by level (stable: replay order within a level); level l + 1 is adds[lvl_begin[l], lvl_begin[l + 1])
     int n_lv = 0;
     for (const PpAdd &a : adds)
-        n_lv = std::max(n_lv, lvl[a.node]);
+        n_lv = std::max(n_lv, nodes[a.node].lvl);
     P.lvl_begin.assign(n_lv + 1, 0);
     for (const PpAdd &a : adds)
-        ++P.lvl_begin[lvl[a.node]];
+        ++P.lvl_begin[nodes[a.node].lvl];
     for (int l = 1; l <= n_lv; ++l)
         P.lvl_begin[l] += P.lvl_begin[l - 1];
     std::vector<int> pos(P.lvl_begin.begin(), P.lvl_begin.end() - 1);
     P.adds.resize(adds.size());
     for (const PpAdd &a : adds)
-        P.adds[pos[lvl[a.node] - 1]++] = a;
+        P.adds[pos[nodes[a.node].lvl - 1]++] = a;
     return P;
 }
 

@@ -29,17 +29,24 @@ namespace da {
 
 enum PsStatus : int { PS_SPLIT = 0, PS_NOT_OK = 1 /* the task is not ok: no split */, PS_KEY_ERROR = 2 /* to_pipeline raises KeyError */, PS_INTERNAL = 3 };
 
+// What an item that is not a network input is (PsItem::inp < 0)
+enum PsKind : int {
+    PS_ADDER = -1,
+    PS_CONSTANT = -2,     // an all-zero output column
+    PS_ONE_OPERAND = -3,  // relu / quantize (opcodes +-2 / +-3), a constant addition (4) or a lookup (8)
+    PS_MUX = -4,          // an MSB mux (opcode +-6)
+};
+
 struct PsItem {
     double lo, hi, step;  // the op's interval (the node's own)
     long long data;       // see x, y, z, opc
     int node, gpos;       // node id (PpDesign) and position in gather_variables' list
-    int inp;              // >= 0: network input k; -1: adder; -2: constant (an all-zero output column); -3: activation;
-                          // -4: MSB mux
-    int x, y, z, opc;     // adder: items of the operands in _from order, opcode, data the shift; activation: the operand's
-                          // item, y -1, opcode +-2 / +-3, data 0; MSB mux: the data operands a, b and the condition z
-                          // (_from is (z, a, b)), opcode +-6, data the shift of b (the written op's data is shift << 32 |
-                          // the condition's row); input: opcode -1, or 5 and the value in steps for an input with a point
-                          // interval (a constant to the tracer).  z is -1 but for a mux.
+    int inp;              // >= 0: network input k; else a PsKind
+    int x, y, z, opc;     // adder: items of the operands in _from order, opcode, data the shift; one-operand op: the
+                          // operand's item, y -1, opcode and data as PpSplitOp; MSB mux: the data operands a, b and the
+                          // condition z (_from is (z, a, b)), opcode +-6, data the shift of b (the written op's data is
+                          // shift << 32 | the condition's row); input: opcode -1, or 5 and the value in steps for an input
+                          // with a point interval (a constant to the tracer).  z is -1 but for a mux.
     int live;             // reachable from the outputs
 };
 
@@ -208,11 +215,11 @@ __global__ void __launch_bounds__(256) pipeline_split_kernel(const PsDesign *des
     // last consumer stage of every item: the stage of each adder reading it, and the output stage
     for (int i = tid; i < M; i += nt) {
         const PsItem &it = D.items[i];
-        if (it.inp == -1 || it.inp == -3 || it.inp == -4)
+        if (it.inp == PS_ADDER || it.inp == PS_ONE_OPERAND || it.inp == PS_MUX)
             atomicMax(&t.last[it.x], t.stg[i]);
-        if (it.inp == -1 || it.inp == -4)
+        if (it.inp == PS_ADDER || it.inp == PS_MUX)
             atomicMax(&t.last[it.y], t.stg[i]);
-        if (it.inp == -4)
+        if (it.inp == PS_MUX)
             atomicMax(&t.last[it.z], t.stg[i]);
     }
     for (int o = tid; o < d.n_out; o += nt)
@@ -270,14 +277,14 @@ __global__ void __launch_bounds__(256) pipeline_split_write_kernel(const PsDesig
     // across every boundary below s: record it at the last one, a suffix min then gives each copy its first event
     for (int i = tid; i < M; i += nt) {
         const PsItem &it = D.items[i];
-        if (it.inp != -1 && it.inp != -3 && it.inp != -4)
+        if (it.inp != PS_ADDER && it.inp != PS_ONE_OPERAND && it.inp != PS_MUX)
             continue;
         const int s = stg[i];
         if (s > stg[it.x])
             atomicMin(&t.ev[coff[it.x] + s - 1 - stg[it.x]], 4 * rank[i]);
-        if (it.inp != -3 && s > stg[it.y])
+        if (it.inp != PS_ONE_OPERAND && s > stg[it.y])
             atomicMin(&t.ev[coff[it.y] + s - 1 - stg[it.y]], 4 * rank[i] + 1);
-        if (it.inp == -4 && s > stg[it.z])
+        if (it.inp == PS_MUX && s > stg[it.z])
             atomicMin(&t.ev[coff[it.z] + s - 1 - stg[it.z]], 4 * rank[i] + 2);
     }
     for (int o = tid; o < n_out; o += nt) {
@@ -335,11 +342,11 @@ __global__ void __launch_bounds__(256) pipeline_split_write_kernel(const PsDesig
                 oi[0] = -1, oi[1] = -1, oi[2] = 5, oi[3] = it.data;
             else if (it.inp >= 0)
                 oi[0] = it.inp, oi[1] = -1, oi[2] = -1, oi[3] = 0;
-            else if (it.inp == -2)
+            else if (it.inp == PS_CONSTANT)
                 oi[0] = -1, oi[1] = -1, oi[2] = 5, oi[3] = 0;
             else {
-                oi[0] = where(it.x, s), oi[1] = it.inp != -3 ? where(it.y, s) : -1, oi[2] = it.opc, oi[3] = it.data;
-                if (it.inp == -4) // to_pipeline's shift << 32 | the condition's row, the shift as its low 32 bits
+                oi[0] = where(it.x, s), oi[1] = it.inp != PS_ONE_OPERAND ? where(it.y, s) : -1, oi[2] = it.opc, oi[3] = it.data;
+                if (it.inp == PS_MUX) // to_pipeline's shift << 32 | the condition's row, the shift as its low 32 bits
                     oi[3] = (int64_t)(((unsigned long long)(unsigned)it.data << 32) | (unsigned long long)where(it.z, s));
                 cost = (double)t.cost[it.node];
             }
@@ -378,40 +385,29 @@ inline PsPrep ps_prepare(const PpPrepared &P, const PpSplitInfo &S) {
     // an op's interval is FixedVariable.unscaled of the view gather_variables met the node through first (its bounds'
     // signs of zero depend on that view's factor); own[node] is set when the walk enters the node
     std::vector<double> own(S.own_q);
-    auto enter = [&](int node, const double *v) { // v: (lo, hi, step, factor); `self * (1 / factor)` in Decimal
-        const double o = 1.0 / v[3], a = v[0] * o, b = v[1] * o;
-        own[3 * (size_t)node] = std::min(a, b), own[3 * (size_t)node + 1] = std::max(a, b), own[3 * (size_t)node + 2] = std::fabs(v[2] * o);
+    auto enter = [&](int node, const PpView &v) { // `self * (1 / factor)` in Decimal
+        const double o = 1.0 / v.f, a = v.lo * o, b = v.hi * o;
+        own[3 * (size_t)node] = std::min(a, b), own[3 * (size_t)node + 1] = std::max(a, b), own[3 * (size_t)node + 2] = std::fabs(v.step * o);
     };
     auto add_item = [&](int node, int gpos) {
         PsItem it{};
         it.node = node, it.gpos = gpos;
         it.lo = own[3 * (size_t)node], it.hi = own[3 * (size_t)node + 1], it.step = own[3 * (size_t)node + 2];
-        it.inp = node < P.n_in ? node : node == CONST ? -2 : -1;
+        it.inp = node < P.n_in ? node : PS_CONSTANT;
         it.x = it.y = it.z = -1;
         it.opc = -1;
         it.live = node < P.n_in ? P.node_bits[node] >= 0 : 1;
         if (it.inp >= 0 && it.lo == it.hi) { // (0, 0, 2^32) for 0, else the step _const_f gives the value
-            int f = -32;
-            if (it.lo != 0) {
-                int lo = -32, hi = 32;
-                while (hi - lo > 1) {
-                    const int mid = lo + (hi - lo) / 2;
-                    const double v = it.lo * std::ldexp(1.0, mid);
-                    (v == std::trunc(v) ? hi : lo) = mid;
-                }
-                f = hi;
-            }
-            it.step = std::ldexp(1.0, -f);
+            it.step = std::ldexp(1.0, -pp_const_f(it.lo));
             it.opc = 5, it.data = (int)(it.lo / it.step);
         }
-        if (it.inp == -1) {
-            const int a = node - P.n_in - 1;
-            it.x = item_of[S.x[a]], it.y = S.y[a] < 0 ? -1 : item_of[S.y[a]];
-            it.opc = S.opc[a], it.data = S.data[a];
-            if (S.y[a] < 0) // relu / quantize
-                it.inp = -3;
-            if (S.z[a] >= 0) // an MSB mux
-                it.inp = -4, it.z = item_of[S.z[a]];
+        if (node > CONST) {
+            const PpSplitOp &op = S.ops[node - CONST - 1];
+            it.inp = op.z.node >= 0 ? PS_MUX : op.y.node >= 0 ? PS_ADDER : PS_ONE_OPERAND;
+            it.x = item_of[op.x.node];
+            it.y = op.y.node < 0 ? -1 : item_of[op.y.node];
+            it.z = op.z.node < 0 ? -1 : item_of[op.z.node];
+            it.opc = op.opc, it.data = op.data;
         }
         Q.items.push_back(it);
         return (int)Q.items.size() - 1;
@@ -425,7 +421,7 @@ inline PsPrep ps_prepare(const PpPrepared &P, const PpSplitInfo &S) {
     struct Entry {
         int node;
         bool done;
-        const double *view;
+        const PpView *view;
     };
     std::vector<Entry> stack;
     std::vector<char> entered(P.n_nodes, 0);
@@ -435,7 +431,7 @@ inline PsPrep ps_prepare(const PpPrepared &P, const PpSplitInfo &S) {
             Q.out_item.push_back(add_item(CONST, pos++));
             continue;
         }
-        stack.assign(1, {root, false, S.out_v.data() + 4 * (size_t)o});
+        stack.assign(1, {root, false, &S.out_v[o]});
         while (!stack.empty()) {
             const Entry e = stack.back();
             const int v = e.node;
@@ -451,16 +447,16 @@ inline PsPrep ps_prepare(const PpPrepared &P, const PpSplitInfo &S) {
                 continue;
             if (!entered[v]) {
                 entered[v] = 1;
-                enter(v, e.view);
+                enter(v, *e.view);
             }
             stack.push_back({v, true, nullptr});
             if (v > CONST) {
-                const int a = v - P.n_in - 1;
-                if (S.y[a] >= 0)
-                    stack.push_back({S.y[a], false, S.yv.data() + 4 * (size_t)a});
-                stack.push_back({S.x[a], false, S.xv.data() + 4 * (size_t)a});
-                if (S.z[a] >= 0) // an MSB mux's _from is (condition, a, b)
-                    stack.push_back({S.z[a], false, S.zv.data() + 4 * (size_t)a});
+                const PpSplitOp &op = S.ops[v - CONST - 1];
+                if (op.y.node >= 0)
+                    stack.push_back({op.y.node, false, &op.y});
+                stack.push_back({op.x.node, false, &op.x});
+                if (op.z.node >= 0) // an MSB mux's _from is (condition, a, b)
+                    stack.push_back({op.z.node, false, &op.z});
             }
         }
         Q.out_item.push_back(item_of[root]);
